@@ -1,8 +1,9 @@
 #!/usr/bin/env python
-"""bench.py -- the UnFlow hot path on N B200s (one process per GPU).
+"""bench.py -- the UnFlow hot path on N H100s (one process per GPU).
 
     python bench.py --gpus N --steps K --warmup W            # this repo's CUDA path
     python bench.py --impl reference --gpus N --steps K ...  # CPU restatement of the reference
+    python bench.py ... --dump-outputs DIR                    # also write what the last timed step computed
 
 Workload ("step" = one pass of the hot path over one batch of synthetic input): the full
 unsupervised FlowNetC training step of BASELINE.json configs[2]/[3] -- bidirectional FlowNetC
@@ -15,14 +16,17 @@ One JSON line on rank 0:
   value   frame-pairs/s, whole job, inputs already resident in HBM when the timed region starts
   e2e     the same metric through the public API (e2eflow ... Trainer.step) with the inputs in
           pinned HOST memory: H2D copy of both frames and D2H read of the loss inside every step
-  roofline  correlation forward kernel: algorithmic bytes / CUDA-event time measured live inside
-          the timed region, against the measured HBM peak (MEASURED_PEAKS.json); extra fields give
-          the fp32-FMA fraction and the same figures for the other hand-written kernels
+  roofline  per hand-written kernel: algorithmic bytes or flops / CUDA-event time measured live in an
+          eager pass, against the H100 SXM data-sheet peaks (or MEASURED_PEAKS.json where present)
   cpu_baseline  (N=1) the CPU oracle (a restatement of the reference -- the reference itself has
           no CPU path for this graph, SURVEY.md R1) on a bounded sample, timed on the host cores
   clocks  nvidia-smi SM clock / throttle reasons sampled (every 100 ms) during the timed region
 Timing: CUDA events on the launching stream, barrier + synchronize on both sides, max over ranks.
-L2: one step streams several GB of activations (>> 126 MB L2), so no explicit flush is needed.
+L2: one step streams several GB of activations (>> 50 MB L2), so no explicit flush is needed.
+--dump-outputs DIR: after the headline timed steps, DIR/<name>.npy holds what the last of them computed --
+the loss and a fixed, seeded sample of the updated parameters and of Adam's first moment (float32 / float64).
+The inputs and the initial weights are seeded, so two builds run with the same arguments can be compared
+output for output.
 """
 import argparse
 import json
@@ -47,7 +51,8 @@ METRIC = "frame-pairs/s at 384x1280 FlowNetC"
 
 
 def load_peaks():
-    peaks = {"hbm_gbs": 6650.0, "sm_max_mhz": 1965.0, "_source": "fallback (B200_PROFILING.md)"}
+    # H100 SXM data sheet (700 W card): 3.35 TB/s HBM3, 989 TFLOP/s dense BF16; SM clock at most 1980 MHz
+    peaks = {"hbm_gbs": 3350.0, "sm_max_mhz": 1980.0, "bf16_tflops": 989.0, "_source": "H100 SXM data sheet"}
     try:
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as fh:
             peaks.update(json.load(fh))
@@ -183,6 +188,8 @@ def run_ours(args):
     if rank == 0:
         sampler.start()          # runs for the whole bench; timed regions pick their samples by time
 
+    last = [None]           # what the latest timed step returned
+
     def timed(fn, steps, hook=False):
         barrier()
         _native.reset_launch_count()
@@ -192,7 +199,7 @@ def run_ours(args):
         t0 = time.time()
         start.record()
         for _ in range(steps):
-            fn()
+            last[0] = fn()
         end.record()
         barrier()
         t1 = time.time()
@@ -208,7 +215,7 @@ def run_ours(args):
         resident_step()
     # eager pass: per-kernel CUDA-event timings for the roofline objects (and the value itself when
     # graphs are off)
-    eager_steps = args.steps if not args.graph else max(3, min(args.steps, 5))
+    eager_steps = args.steps if not args.graph else min(args.steps, 5)
     ms, launches, ktimes, clocks = timed(resident_step, eager_steps, hook=True)
     kbytes = dict(ops.kernel_timer.bytes)
     steps_timed = eager_steps
@@ -220,6 +227,8 @@ def run_ours(args):
         ms, _, _, clocks = timed(resident_step, args.steps)
         launches = trainer._graph_launches * args.steps
         steps_timed = args.steps
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, trainer, last[0])
 
     def e2e_step():   # host batch -> (static) device buffers, step, loss back to the host
         if args.graph:
@@ -273,7 +282,7 @@ def run_ours(args):
     pairs = PER_GPU_BATCH * world * args.steps
     value = PER_GPU_BATCH * world * steps_timed / (ms * 1e-3)
     e2e = pairs / (ms_e2e * 1e-3)
-    fma_peak = 148 * 128 * 2 * peaks["sm_max_mhz"] * 1e6 / 1e12
+    fma_peak = 132 * 128 * 2 * peaks["sm_max_mhz"] * 1e6 / 1e12       # 132 SMs x 128 fp32 lanes x FMA
 
     def roof(name, nbytes=None, flops=None):
         t = ktimes.get(name)
@@ -285,7 +294,7 @@ def run_ours(args):
         r = {"kernel": name, "bound": "hbm", "launches_timed": len(t), "avg_us": round(avg * 1e6, 2),
              "achieved": round(nbytes / avg / 1e9, 1), "peak": peaks["hbm_gbs"], "unit": "GB/s",
              "frac": round(nbytes / avg / 1e9 / peaks["hbm_gbs"], 4), "peak_source": peaks["_source"],
-             "algorithmic_bytes": nbytes, "traffic": TRAFFIC.get(name)}
+             "algorithmic_bytes": nbytes}
         if flops:
             r["fp32_tflops"] = round(flops / avg / 1e12, 2)
             r["fma_frac"] = round(flops / avg / 1e12 / fma_peak, 4)
@@ -296,9 +305,9 @@ def run_ours(args):
     corr_flops = 2 * Bc * hc * wc * C * D2
     npx0 = PER_GPU_BATCH * (H // 4) * (W // 4)
     # tensor-core conv kernels: nominal flops (2 x multiply-adds of the fp32 convolution) are executed as
-    # three TF32 MMA passes (hi*hi + hi*lo + lo*hi); the tensor roofline is the measured sustained bf16
-    # GEMM rate / 2 (TF32 has half the bf16 MMA rate)
-    tf32_peak = peaks.get("bf16_tflops_sustained", 1442.1) / 2.0
+    # three TF32 MMA passes (hi*hi + hi*lo + lo*hi); the tensor roofline is the bf16 rate / 2 (TF32 has
+    # half the bf16 MMA rate)
+    tf32_peak = peaks.get("bf16_tflops_sustained", peaks["bf16_tflops"]) / 2.0
 
     def tensor_roof(name, label):
         t = ktimes.get(name)
@@ -310,13 +319,13 @@ def run_ours(args):
         return {"kernel": label, "bound": "tensor", "launches_timed": len(t),
                 "avg_us": round(total_ms / len(t) * 1e3, 2), "achieved": round(3 * nominal, 1),
                 "peak": round(tf32_peak, 1), "unit": "TFLOP/s", "frac": round(3 * nominal / tf32_peak, 4),
-                "peak_source": peaks["_source"] + ": bf16_tflops_sustained / 2 (TF32)",
+                "peak_source": peaks["_source"] + ": bf16 / 2 (TF32)",
                 "nominal_fp32_tflops": round(nominal, 1), "mma_passes_per_product": 3,
-                "algorithmic_flops": int(flops // max(len(t), 1)), "traffic": TRAFFIC.get(name),
+                "algorithmic_flops": int(flops // max(len(t), 1)),
                 "ms_per_step": round(total_ms / max(steps_timed_eager, 1), 3)}
 
-    roofs = [tensor_roof("tc_conv", "tc_conv_kernel (tcgen05 3xTF32 conv / deconv forward + input gradient, all launches)"),
-             tensor_roof("tc_wgrad", "tc_wgrad_kernel (tcgen05 3xTF32 weight gradient, all launches)"),
+    roofs = [tensor_roof("tc_conv", "tc_conv_kernel (wgmma 3xTF32 conv / deconv forward + input gradient, all launches)"),
+             tensor_roof("tc_wgrad", "tc_wgrad_kernel (wgmma 3xTF32 weight gradient, all launches)"),
              # one-pass bidirectional correlation: inputs read once, both volumes written (+ the zero fill of the
              # reverse volume); flops = the ONE set of products both volumes share
              roof("correlation_fwd_bidir", 4 * Bc * hc * wc * (2 * C + 3 * D2), corr_flops),
@@ -341,9 +350,9 @@ def run_ours(args):
                          % (args.spec, args.batch)),
                    "flownet": args.spec,
                    "global_batch": PER_GPU_BATCH * world, "parallelism": "dp%d" % world,
-                   "l2": "inputs+activations per step >> 126 MB L2 (no flush needed)",
+                   "l2": "inputs+activations per step >> 50 MB L2 (no flush needed)",
                    "conv_precision": ("fp32 (cuDNN, TF32 disabled)" if args.conv == "fp32" else
-                                      "3xTF32 split on tensor cores, hand-written tcgen05 kernels with fp32 register "
+                                      "3xTF32 split on tensor cores, hand-written wgmma kernels with fp32 register "
                                       "accumulation (2e-6 vs float64 per layer, parity-tested)"),
                    "cudnn_benchmark": bool(args.cudnn_benchmark),
                    "cuda_graph": bool(args.graph)},
@@ -378,13 +387,22 @@ def _finish(world):
         os._exit(0)
 
 
-# measured once with `ncu --set full` (profiles/): dram__bytes_read.sum + dram__bytes_write.sum per launch
-TRAFFIC = {}
-try:
-    with open(os.path.join(ROOT, "profiles", "dram_traffic.json")) as _fh:
-        TRAFFIC = json.load(_fh)
-except Exception:
-    pass
+DUMP_SAMPLE = 1 << 22      # elements kept of each large output (16 MB of float32)
+
+
+def dump_outputs(out_dir, trainer, loss):
+    """Write what the last timed step computed: the loss it returned and a fixed, seeded sample of the
+    parameters it updated and of Adam's first moment (the step's gradient, averaged).  The sample positions
+    are sorted(numpy.random.default_rng(0).choice(n_parameters, DUMP_SAMPLE, replace=False))."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    torch.cuda.synchronize()
+    n = trainer.flat_param.numel()
+    idx = torch.from_numpy(np.sort(np.random.default_rng(0).choice(n, min(n, DUMP_SAMPLE), replace=False)))
+    idx = idx.to(trainer.flat_param.device)
+    np.save(os.path.join(out_dir, "loss.npy"), np.asarray(float(loss), dtype=np.float64))
+    np.save(os.path.join(out_dir, "param_sample.npy"), trainer.flat_param[idx].cpu().numpy())
+    np.save(os.path.join(out_dir, "adam_m_sample.npy"), trainer.adam_m[idx].cpu().numpy())
 
 
 # ---------------------------------------------------------------------------------------------
@@ -492,6 +510,8 @@ def main():
     ap.add_argument("--also-fp32", type=int, nargs="?", const=1, default=1,
                     help="1 (default, N=1 only): additionally time the exact-fp32 conv mode (no tensor "
                          "cores) for a few steps and report it as fp32_exact next to the 3xTF32 headline")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps, write what the last one computed to DIR/<name>.npy")
     args = ap.parse_args()
     if args.impl == "reference":
         run_reference(args)

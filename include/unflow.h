@@ -1,5 +1,5 @@
 /*
- * unflow.h -- C ABI of libunflow.so, the sm_100a kernels behind the UnFlow hot path.
+ * unflow.h -- C ABI of libunflow.so, the sm_90a kernels behind the UnFlow hot path.
  *
  * This is the drop-in boundary: the reference binds its ops through
  * TensorFlow's C++ OpKernel interface (tf.load_op_library, reference
@@ -51,7 +51,10 @@ const char *unflow_last_error(void);
 unsigned long long unflow_launch_count(void);
 void unflow_reset_launch_count(void);
 /* Tuning knobs for tests / benchmarks.  "corr_fwd_variant": 1 (one row pair per thread) or
- * 3 (three row pairs per thread); default 1 (faster on B200); results are bit-identical. */
+ * 3 (three row pairs per thread); default 1; results are bit-identical.  "tc_chunk" (1..64): K blocks per
+ * tensor-core accumulation of the tc_* kernels; "tc_ksplit" (0 / 1): split the K loop of layers with few
+ * tiles; "tc_pair_px" (0 / 1): two output-parity classes per tile in narrow transposed layers;
+ * "narrow_fwd_tma" (0 / 1): TMA-staged narrow 3x3 forward. */
 int unflow_set_int_option(const char *name, int value);
 
 /* ------------------------------------------------------------------------
@@ -272,11 +275,11 @@ int unflow_conv3x3_narrow_wgrad(const float *x, long long x_pitch, const float *
 
 /* ---- conv / deconv stacks on the tensor cores (csrc/tc_conv.cu) --------------------------------
  * The reference's slim.conv2d / slim.conv2d_transpose layers (src/e2eflow/core/flownet.py:166-233,
- * _flownet_upconv :89-155; cuDNN behind TensorFlow) as a hand-written tcgen05 implicit GEMM:
+ * _flownet_upconv :89-155; cuDNN behind TensorFlow) as a hand-written wgmma implicit GEMM:
  * fp32 activations are read from HBM once (TMA), split into TF32 hi / lo planes in shared memory,
- * three kind::tf32 MMAs per K step accumulate in tensor memory (fp32-level accuracy, "3xTF32"),
+ * three tf32 wgmma per K step accumulate in registers (fp32-level accuracy, "3xTF32"),
  * the epilogue adds the bias, applies max(slope*x, x) (flownet.py:84-86) and writes -- or, with
- * `accumulate`, adds -- float4 vectors into the destination.
+ * `accumulate`, adds -- into the destination.
  *
  * unflow_tc_wsplit: weight planes hi = tf32(w), lo = w - hi in the layout [taps][R][Cp]
  *   (R = the GEMM's output channels, C = contraction channels, Cp = C rounded up to 4, tail zero);
@@ -289,11 +292,8 @@ int unflow_conv3x3_narrow_wgrad(const float *x, long long x_pitch, const float *
  *           (slim.conv2d; TF SAME padding enters as the offsets pad_t / pad_l, zero outside)
  *   mode 1  y[stride*iy - pad_t + ky, stride*ix - pad_l + kx] += x[iy,ix] W[ky*kw+kx]
  *           (slim.conv2d_transpose and the input gradient of mode 0; Hout, Wout % stride == 0)
- *   stride 1 or 2, kh*kw <= 64.  UNFLOW_EINVAL otherwise.
- *   mode | 2: the weight planes are those of the layer's other direction, [taps][Cin][Cout_p] (contraction
- *           outermost): the input gradient of a layer reuses the planes its forward pass split, no second,
- *           transposed pair of planes is made (the kernel then reads B tiles MN-major). */
-/* Debug hook (tools/tc_conv_check.py --roles): CTA 0 of every following tc_conv launch writes its role timers
+ *   stride 1 or 2, kh*kw <= 64.  UNFLOW_EINVAL otherwise. */
+/* Debug hook: CTA 0 of every following tc_conv launch writes its role timers
  * (clocks blocked on each pipeline barrier / in total, see csrc/tc_conv.cu) into `buf`, device memory for 16
  * long longs; nullptr switches it off. */
 int unflow_tc_conv_debug(long long *buf);
@@ -311,7 +311,7 @@ int unflow_tc_conv(const float *x, int N, int Hin, int Win, int Cin, long long x
                    int mode, int stride, int kh, int kw, int pad_t, int pad_l, void *stream);
 
 /* unflow_tc_wgrad (csrc/tc_wgrad.cu): weight gradient of the same layers, same arithmetic (both operands
- * split in shared memory, MN-major tcgen05 operands straight from the NHWC activations, fp32 register
+ * split and transposed in shared memory straight from the NHWC activations, wgmma, fp32 register
  * accumulation, split-K):
  *     dw[r * pitch_r + t * pitch_t + c] += sum_p P[p][r] * G[stride * p + (k - pad)][c],   t = ky*kw + kx
  *   slim.conv2d:            P = dL/dy [N,Hp,Wp,R=C_out],  G = x     [N,Hg,Wg,C=C_in]

@@ -1,14 +1,15 @@
 """The reference's OWN CUDA kernels as a checker (TEST INFRASTRUCTURE ONLY).
 
 ``oracle/ref_ops/build.sh`` compiles /root/reference/ops/{correlation,backward_warp,forward_warp,
-downsample}_op.cu.cc for sm_100a exactly as they lie in the reference tree -- nothing is copied --
+downsample}_op.cu.cc for sm_90a exactly as they lie in the reference tree -- nothing is copied --
 against stand-in headers (oracle/tf_stub) for the handful of TensorFlow declarations those files
 include, and links them with a C wrapper (oracle/ref_ops/wrapper.cu) into oracle/_ref/libref_ops.so.
 The op-registration files (*_op.cc) need the whole TensorFlow op framework and are not built; by
 the letter of the task the reference is therefore "unbuildable", what IS built are its GPU kernels
 and their launchers, which is where the arithmetic lives.
 
-Used by tests/test_reference_kernels.py (every ``-m gpu`` run) and tools/bench_reference_kernels.py.
+Used by tests/golden/make_reference_kernels.py, which stores what tests/test_reference_kernels.py compares
+against, and by tools/bench_reference_kernels.py.
 
 All functions take / return float32 CUDA tensors in the reference's layouts (correlation NCHW, the
 warps and downsample NHWC) and synchronise before returning; the kernels run on the legacy default
@@ -26,12 +27,9 @@ _lib = None
 
 
 def build():
-    """(Re)build when the reference tree is present (the build container) and fail loudly if that
-    leaves no library; where the tree is absent (the GPU box) the prebuilt file must have travelled."""
+    """(Re)build when the reference tree is present (UNFLOW_REFERENCE, see ref_ops/build.sh); without it
+    nothing is built -- the tests read the stored golden vectors only."""
     subprocess.check_call(["bash", os.path.join(HERE, "ref_ops", "build.sh")])
-    if not available():
-        raise RuntimeError("%s is missing: the reference kernels are the GPU ground truth of the "
-                           "parity tests (oracle/ref_ops/build.sh needs /root/reference)" % LIB_PATH)
 
 
 def available():

@@ -19,13 +19,13 @@ if [ -f "$LIB" ] && [ -z "$UNFLOW_FORCE_BUILD" ]; then
   [ $stale -eq 0 ] && { echo "up to date: $LIB"; exit 0; }
 fi
 unset CC CXX
-FLAGS="-gencode arch=compute_100a,code=sm_100a -O2 -lineinfo -std=c++17 -DGOOGLE_CUDA=1 -Xcompiler -fPIC -I $ORACLE/tf_stub -I $REF/ops"
+FLAGS="-gencode arch=compute_90a,code=sm_90a -O2 -lineinfo -std=c++17 -DGOOGLE_CUDA=1 -Xcompiler -fPIC -I $ORACLE/tf_stub -I $REF/ops"
 OBJS=""
 for f in correlation_op backward_warp_op forward_warp_op downsample_op; do
   "$NVCC" $FLAGS -x cu -c "$REF/ops/$f.cu.cc" -o "$OUT/$f.o"
   OBJS="$OBJS $OUT/$f.o"
 done
 "$NVCC" $FLAGS -c "$HERE/wrapper.cu" -o "$OUT/wrapper.o"
-"$NVCC" -shared -o "$OUT/libref_ops.so" $OBJS "$OUT/wrapper.o" -gencode arch=compute_100a,code=sm_100a -Xcompiler -fPIC
+"$NVCC" -shared -o "$OUT/libref_ops.so" $OBJS "$OUT/wrapper.o" -gencode arch=compute_90a,code=sm_90a -Xcompiler -fPIC
 rm -f $OBJS "$OUT/wrapper.o"
 echo "built $OUT/libref_ops.so"

@@ -29,6 +29,8 @@ sys.path.insert(0, HERE)
 REF_SRC = os.environ.get("UNFLOW_REFERENCE_SRC", "/root/reference/src")
 
 import tf_shim  # noqa: E402
+sys.path.insert(0, os.path.dirname(HERE))
+import synth as synth_tests  # noqa: E402
 from oracle import flownet as oflownet  # noqa: E402
 from oracle import ops as oops  # noqa: E402
 from unflow_b200 import synthetic as synth  # noqa: E402
@@ -321,8 +323,26 @@ def main():
     out['restore_plans_json'] = np.array(json.dumps(plans))
 
     path = os.path.join(HERE, 'reference_run.npz')
-    np.savez_compressed(path, **out)
+    np.savez_compressed(path, **shrink(out))
     print("wrote %s: %d arrays, %.1f KB" % (path, len(out), os.path.getsize(path) / 1024.0))
+
+
+def shrink(out):
+    """What is stored (tests/synth.py, ReferenceRun): no image pairs of tests/synth.py RUN_IMAGES (the tests
+    redraw them from their seeds -- checked here), the output flows of unsupervised_loss at RUN_SAMPLE seeded
+    positions with their shape and largest magnitude."""
+    out = dict(out)
+    for tag in synth_tests.RUN_IMAGES:
+        for i, want in enumerate(synth_tests.run_images(tag)):
+            assert np.array_equal(out.pop('%s_im%d' % (tag, i + 1)), want), tag
+    for key in [k for k in out if k.startswith('ul_') and '_flow_' in k]:
+        v = np.asarray(out.pop(key))
+        idx = np.sort(np.random.default_rng(sum(map(ord, key))).choice(v.size, synth_tests.RUN_SAMPLE, replace=False))
+        out[key + '_shape'] = np.asarray(v.shape, dtype=np.int64)
+        out[key + '_absmax'] = np.float64(np.abs(v).max())
+        out[key + '_idx'] = idx.astype(np.int64)
+        out[key + '_val'] = v.reshape(-1)[idx]
+    return out
 
 
 if __name__ == '__main__':

@@ -184,7 +184,7 @@ def test_narrow_flow_head_matches_float64(mode3x, N, C, H, W):
     y2 = conv_ops._NarrowConv3x3.apply(xc.detach(), wc2, bc.detach())
     y2.backward(gc)
     assert torch.equal(wc2.grad, wc.grad)
-    if N * ((H + 15) // 16) * ((W + 31) // 32) >= 2 * 148:
+    if N * ((H + 15) // 16) * ((W + 31) // 32) >= 2 * 132:      # 132 SMs (H100 SXM)
         assert torch.equal(y2, y)
     else:
         assert rel(y2.detach().cpu(), y.detach().cpu()) < 1e-6
@@ -263,7 +263,7 @@ def test_narrow_conv_on_a_channel_slice_of_a_wider_buffer(mode3x):
         y = conv_ops._NarrowConv3x3.apply(x, wr, b)
         y.backward(g)
         outs.append((y.detach().clone(), wr.grad.clone()))
-    # 18 tiles < 2 x 148 SMs: the forward splits the channels over several CTAs that add their parts with
+    # 18 tiles < 2 x 132 SMs: the forward splits the channels over several CTAs that add their parts with
     # atomics (order not fixed), the weight gradient splits them into disjoint ranges (bit-identical)
     # (the dense copy has a pixel pitch of 194 floats, which TMA cannot address: it runs on the cp.async kernels,
     # the pitch-200 slice on the TMA-staged ones -- same sums in another order)

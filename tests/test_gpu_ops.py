@@ -1,5 +1,5 @@
 """GPU parity of the four custom ops, called through the reference-style Python surface
-(unflow_b200.e2eflow.ops -> ctypes -> C ABI -> sm_100a kernels), against the CPU oracle on the
+(unflow_b200.e2eflow.ops -> ctypes -> C ABI -> sm_90a kernels), against the CPU oracle on the
 same seeded inputs and against the reference's own known-answer vectors."""
 import numpy as np
 import pytest

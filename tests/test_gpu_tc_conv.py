@@ -1,4 +1,4 @@
-"""The hand-written tcgen05 convolution kernels (csrc/tc_conv.cu, csrc/tc_wgrad.cu) through the C ABI
+"""The hand-written wgmma convolution kernels (csrc/tc_conv.cu, csrc/tc_wgrad.cu) through the C ABI
 against float64 convolutions: every mode the FlowNet stacks use -- slim.conv2d with TF SAME padding at
 stride 1 / 2, slim.conv2d_transpose (k4 s2), the input gradients of both, the weight gradients, the
 row-window form of the 7x7 first layers -- including ragged channel counts, channel-sliced (pitched)
@@ -209,7 +209,7 @@ def test_first_layer_row_window_form(Ci, H, W):
 
 def test_conv_ops_layers_run_on_the_tensor_core_kernels():
     """conv_ops.conv2d / conv_transpose2d in 3xTF32 mode: values and all three gradients of a conv and a
-    deconv layer against float64 autograd, and the launch counter proves the tcgen05 kernels ran."""
+    deconv layer against float64 autograd, and the launch counter proves the wgmma kernels ran."""
     from unflow_b200 import _native
     from unflow_b200.e2eflow.core import conv_ops
     prev = conv_ops.get_mode()
@@ -255,3 +255,36 @@ def test_lrelu_bwd_bias_pass(C, hw, act_pitch):
     assert float((gpre.double() - want).abs().max()) <= 1e-6 * float(want.abs().max())
     wb = want.sum((0, 2, 3))
     assert float((gb.double() - wb).abs().max()) <= 2e-6 * float(want.abs().sum((0, 2, 3)).max())
+
+
+def test_launch_from_a_fresh_host_thread():
+    """A host thread whose first CUDA call is one of the library's launchers -- autograd's backward worker running
+    the correlation gradient, for one -- has no current context until something binds the device's primary
+    context; the tensor-map encode inside the launcher has to do that itself (it failed with
+    CUDA_ERROR_INVALID_CONTEXT).  Everything is prepared on the main thread, the launch happens on a new one."""
+    import threading
+    from unflow_b200 import _native
+    tc = T()
+    N, C, H, W = 2, 64, 16, 24
+    g = torch.Generator().manual_seed(17)
+    x = tc.empty_nhwc(N, C, H, W, "cuda")
+    x.copy_(torch.randn(N, C, H, W, generator=g))
+    w = torch.randn(C, 3, 3, C, generator=g).permute(0, 3, 1, 2).cuda()        # [Co][kh][kw][Ci] memory
+    planes = tc.split_weights(w)
+    want, got = tc.empty_nhwc(N, C, H, W, "cuda"), tc.empty_nhwc(N, C, H, W, "cuda")
+    tc.run(x, planes, want, mode=0, stride=1, kh=3, kw=3, pad_t=1, pad_l=1)
+    torch.cuda.synchronize()
+    lib = _native.lib()
+    xp, yp = tc.nhwc_geometry(x)[4], tc.nhwc_geometry(got)[4]
+    result = {}
+
+    def launch():
+        result["rc"] = lib.unflow_tc_conv(x.data_ptr(), N, H, W, C, xp, planes.hi.data_ptr(), planes.lo.data_ptr(),
+                                          got.data_ptr(), H, W, C, yp, None, 0.1, 0, 0, 0, 1, 3, 3, 1, 1, None)
+        result["err"] = _native.last_error()
+    t = threading.Thread(target=launch)
+    t.start()
+    t.join()
+    assert result["rc"] == 0, result["err"]
+    torch.cuda.synchronize()
+    assert torch.equal(got, want)

@@ -1,8 +1,8 @@
 #!/usr/bin/env python
-"""Op-level timing on one B200 (CUDA events, L2 flushed between iterations).
+"""Op-level timing on one H100 (CUDA events, L2 flushed between iterations).
 
 Prints one JSON line per kernel with the algorithmic bytes / FLOPs of SURVEY.md 8d and the
-achieved fraction of the measured peaks (MEASURED_PEAKS.json)."""
+achieved fraction of the H100 SXM data-sheet peaks (or MEASURED_PEAKS.json where present)."""
 import json
 import os
 import sys
@@ -14,12 +14,12 @@ sys.path.insert(0, ROOT)
 from unflow_b200.e2eflow import ops  # noqa: E402
 from unflow_b200.e2eflow.core.image_warp import image_warp  # noqa: E402
 
-PEAKS = {"hbm_gbs": 6650.0, "sm_max_mhz": 1965.0}
+PEAKS = {"hbm_gbs": 3350.0, "sm_max_mhz": 1980.0}      # H100 SXM data sheet
 try:
     PEAKS.update(json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json"))))
 except Exception:
     pass
-FMA_PEAK = 148 * 128 * 2 * PEAKS["sm_max_mhz"] * 1e6 / 1e12  # TFLOP/s fp32
+FMA_PEAK = 132 * 128 * 2 * PEAKS["sm_max_mhz"] * 1e6 / 1e12  # TFLOP/s fp32
 
 
 def timeit(fn, iters=20, warmup=5, flush=True):

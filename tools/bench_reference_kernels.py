@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Op-level timing of the reference's own CUDA kernels (oracle/_ref/libref_ops.so, see
-oracle/ref_kernels.py) next to this repository's kernels, same inputs, one B200:
+oracle/ref_kernels.py) next to this repository's kernels, same inputs, one H100:
 
     python tools/bench_reference_kernels.py        (prints one JSON line per op)
 

@@ -2,9 +2,8 @@
 """Per-kernel GPU time of ONE warm training step (CUPTI activity records through torch.profiler):
 kernel name, launches, total time, share of the step -- as a markdown table on stdout.
 
-Complements the ncu launch lists under profiles/: ncu serialises and replays every launch with a
-cold cache (about 0.17 s per launch for this step), CUPTI's activity trace costs nothing per
-launch and times the kernels warm, in the order and overlap the step really has."""
+CUPTI's activity trace costs little per launch and times the kernels warm, in the order and
+overlap the step really has."""
 import collections
 import os
 import re

@@ -1,4 +1,4 @@
-"""unflow_b200 -- B200-native (sm_100a) implementation of the UnFlow hot path.
+"""unflow_b200 -- H100-native (sm_90a) implementation of the UnFlow hot path.
 
 Layout:
   csrc/        hand-written CUDA kernels + the C ABI (include/unflow.h) -> libunflow.so

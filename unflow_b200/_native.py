@@ -87,7 +87,7 @@ def lib():
         return _lib
     if not os.path.exists(LIB_PATH):
         raise NativeLibraryError(
-            "%s not found: build it with `python -m unflow_b200.build` (nvcc, sm_100a). "
+            "%s not found: build it with `python -m unflow_b200.build` (nvcc, sm_90a). "
             "There is no CPU / PyTorch fallback for the UnFlow ops." % LIB_PATH)
     try:
         handle = ctypes.CDLL(LIB_PATH)

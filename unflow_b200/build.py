@@ -1,4 +1,4 @@
-"""Build libunflow.so (the C-ABI CUDA library) in-tree with nvcc for sm_100a.
+"""Build libunflow.so (the C-ABI CUDA library) in-tree with nvcc for sm_90a.
 
 The reference JIT-compiles each op with nvcc + g++ against TensorFlow headers
 (reference src/e2eflow/ops.py:21-48); here one shared library holds every kernel and
@@ -14,7 +14,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libunflow.so")
 SOURCES = ["abi.cu", "correlation.cu", "correlation_tiled.cu", "warp.cu", "forward_warp.cu",
            "downsample.cu", "level_loss.cu", "adam.cu", "split.cu", "checksum.cu", "narrow_conv.cu", "tc_conv.cu", "tc_wgrad.cu", "relayout.cu", "narrow_conv_tma.cu"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"]
 
 
@@ -57,7 +57,7 @@ def build(force=False, verbose=False):
             sys.stdout.write(out.decode())
         if p.returncode != 0:
             raise RuntimeError("nvcc failed on %s" % src)
-    cmd = [_nvcc(), "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_100a,code=sm_100a",
+    cmd = [_nvcc(), "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_90a,code=sm_90a",
                                                     "-Xcompiler", "-fPIC"]
     subprocess.check_call(cmd, env=env)
     return LIB

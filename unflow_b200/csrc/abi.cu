@@ -15,13 +15,9 @@ void set_error(const char *fmt, ...) {
   vsnprintf(g_err, sizeof(g_err), fmt, ap);
   va_end(ap);
 }
-int set_tc_a_tmem(int v);       // tc_conv.cu
-int set_tc_pair(int v);         // tc_conv.cu
 int set_tc_chunk(int v);        // tc_conv.cu
 int set_tc_ksplit(int v);       // tc_conv.cu
 int set_tc_pair_px(int v);      // tc_conv.cu
-int set_tc_wgrad_gsplit(int v); // tc_wgrad.cu
-int set_tc_wgrad_trunc(int v);  // tc_wgrad.cu
 int set_narrow_fwd_tma(int v);  // narrow_conv.cu
 void count_launch(int n) { g_launches.fetch_add((unsigned long long)n, std::memory_order_relaxed); }
 }  // namespace unflow
@@ -36,13 +32,9 @@ int unflow_set_int_option(const char *name, int value) {
     unflow::g_corr_fwd_variant = value;
     return UNFLOW_OK;
   }
-  if (name && !strcmp(name, "tc_a_tmem") && unflow::set_tc_a_tmem(value)) return UNFLOW_OK;
-  if (name && !strcmp(name, "tc_pair") && unflow::set_tc_pair(value)) return UNFLOW_OK;
   if (name && !strcmp(name, "tc_chunk") && unflow::set_tc_chunk(value)) return UNFLOW_OK;
   if (name && !strcmp(name, "tc_ksplit") && unflow::set_tc_ksplit(value)) return UNFLOW_OK;
   if (name && !strcmp(name, "tc_pair_px") && unflow::set_tc_pair_px(value)) return UNFLOW_OK;
-  if (name && !strcmp(name, "tc_wgrad_gsplit") && unflow::set_tc_wgrad_gsplit(value)) return UNFLOW_OK;
-  if (name && !strcmp(name, "tc_wgrad_trunc") && unflow::set_tc_wgrad_trunc(value)) return UNFLOW_OK;
   if (name && !strcmp(name, "narrow_fwd_tma") && unflow::set_narrow_fwd_tma(value)) return UNFLOW_OK;
   unflow::set_error("unknown option or value: %s=%d", name ? name : "(null)", value);
   return UNFLOW_EINVAL;

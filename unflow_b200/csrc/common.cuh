@@ -1,4 +1,4 @@
-// common.cuh -- shared host/device helpers for libunflow.so (sm_100a only).
+// common.cuh -- shared host/device helpers for libunflow.so (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <cstdarg>
@@ -31,12 +31,27 @@ inline int check_launch(const char *what) {
     }                                  \
   } while (0)
 
-constexpr int kNumSMs = 148;  // B200
+constexpr int kNumSMs = 132;  // H100 SXM
+
+// cuTensorMapEncodeTiled is a driver-API call and needs a current context on the calling thread.  A host thread
+// whose first CUDA work is a launcher of this library (autograd's backward worker, for one) has none until a
+// runtime call binds the device's primary context, and the encode then fails with CUDA_ERROR_INVALID_CONTEXT.
+// cudaSetDevice binds it.  Call this before encoding a tensor map.
+inline int bind_primary_context() {
+  int dev = 0;
+  cudaError_t e = cudaGetDevice(&dev);
+  if (e == cudaSuccess) e = cudaSetDevice(dev);
+  if (e != cudaSuccess) {
+    set_error("cannot make the device's primary context current: %s", cudaGetErrorString(e));
+    return UNFLOW_ECUDA;
+  }
+  return UNFLOW_OK;
+}
 
 inline int ceil_div(long long a, long long b) { return (int)((a + b - 1) / b); }
 
 // grid size for a grid-stride pixel-parallel kernel: enough CTAs to fill the
-// 148 SMs a whole number of times, capped by the work available.
+// SMs a whole number of times, capped by the work available.
 inline int grid_for(long long work_items, int threads, int ctas_per_sm = 8) {
   long long need = (work_items + threads - 1) / threads;
   long long cap = (long long)kNumSMs * ctas_per_sm;

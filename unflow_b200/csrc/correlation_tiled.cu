@@ -1,4 +1,4 @@
-// correlation_tiled.cu -- the FlowNetC cost volume on sm_100a: TMA-staged, register-tiled fp32.
+// correlation_tiled.cu -- the FlowNetC cost volume on sm_90a: TMA-staged, register-tiled fp32.
 //
 // Serves kernel_size=1, stride_1=1, stride_2=2, pad == max_displacement <= 20, H even, W % 4 == 0
 // (reference call site src/e2eflow/core/flownet.py:221-222; math of CorrelateData,
@@ -69,7 +69,7 @@ struct Smem {
 }  // namespace ct
 
 // ------------------------------------------------------------------------------------------
-// PTX helpers (mbarrier + TMA), sm_100a
+// PTX helpers (mbarrier + TMA), sm_90a
 // ------------------------------------------------------------------------------------------
 __device__ __forceinline__ unsigned smem_u32(const void *p) {
   return (unsigned)__cvta_generic_to_shared(p);
@@ -332,8 +332,8 @@ corr_fold_grad_kernel(const float *__restrict__ g, const float *__restrict__ gre
 // ------------------------------------------------------------------------------------------
 // Forward kernel, variant 2: three row pairs per thread.
 //
-// Variant 1 issues 9 LDS.128 per 88 FMAs (9.8 FMA per 128-bit shared load); measured on B200 it
-// sits at ~43 % of the fp32 peak with the shared-memory pipe as the limiter (a 128-bit warp load
+// Variant 1 issues 9 LDS.128 per 88 FMAs (9.8 FMA per 128-bit shared load), which makes the shared-memory
+// pipe the limiter rather than the FMA pipe (a 128-bit warp load
 // costs 4 wavefronts even when lanes share addresses, so >= 16 FMA per LDS.128 are needed to be
 // FMA-bound).  Here a thread owns THREE row pairs that share the in1 row (y, y-2, y-4 against the
 // same y2, i.e. p, p+1, p+2), 4 pixels and 11 displacements: the 24-float in1 window is loaded once
@@ -556,6 +556,7 @@ static EncodeTiledFn get_encode_fn() {
 
 static int encode_map(CUtensorMap *m, const float *base, int rank, const cuuint64_t *dims,
                       const cuuint64_t *strides_bytes, const cuuint32_t *box) {
+  if (bind_primary_context()) return UNFLOW_ECUDA;
   EncodeTiledFn fn = get_encode_fn();
   if (!fn) { set_error("cuTensorMapEncodeTiled entry point not available"); return UNFLOW_ECUDA; }
   cuuint32_t estr[5] = {1, 1, 1, 1, 1};
@@ -566,7 +567,7 @@ static int encode_map(CUtensorMap *m, const float *base, int rank, const cuuint6
   return UNFLOW_OK;
 }
 
-int g_corr_fwd_variant = 1;   // measured: v1 0.429 ms, v3 0.486 ms at B=8 (fewer warps hide less latency)
+int g_corr_fwd_variant = 1;   // v3 runs fewer warps, which hide less latency
 
 bool corr_tiled_supported(const CorrGeom &g) {
   return g.ks == 1 && g.s1 == 1 && g.s2 == ct::S2 && g.pad == g.md && g.ngr <= ct::RMAX &&

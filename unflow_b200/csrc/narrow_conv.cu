@@ -55,8 +55,6 @@ __device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wai
 // consecutive pixels x 16 channels = two 64-byte runs; out-of-image / beyond-C elements are
 // zero-filled by a copy of size 0.  The copies are issued row by row: the row pointer and the bounds
 // test of a window row are computed once, the columns of a thread are a fixed unrolled set.
-// (Round 2 A/B on B200, same lease: this loader 21.43 ms/step, the per-pixel cp.async loop 21.80, the
-// synchronous float2 loader slower still -- the two losers were removed, profiles/r2_ab.md.)
 template <int CHS, int PITCH_>
 __device__ __forceinline__ void stage(float *xs, const float *__restrict__ x, int n, int y0, int x0, int c0,
                                       int H, int W, int C, long long XP, int tid) {
@@ -99,7 +97,7 @@ narrow_fwd_kernel(const float *__restrict__ x, const float *__restrict__ w, cons
   extern __shared__ __align__(16) float smem[];
   float *xs = smem;                           // [KC][CHS]
   float *ws = smem + KC * CHS;                // [KC][3][8]: co0 kx0..2, co1 kx0..2, 0, 0
-  // csplit > 1 (small images: flow4..flow6 have 8..48 tiles for 148 SMs): blockIdx.z also selects a slice of
+  // csplit > 1 (small images: flow4..flow6 have 8..48 tiles for 132 SMs): blockIdx.z also selects a slice of
   // the input channels; the slices' partial sums meet in y (zeroed by the launcher) through atomics
   const int tid = threadIdx.x, n = blockIdx.z / csplit, split = blockIdx.z - n * csplit;
   const int y0 = blockIdx.y * TH, x0 = blockIdx.x * TW;

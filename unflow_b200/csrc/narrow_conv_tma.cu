@@ -11,7 +11,7 @@
 //   pixels x 64 B under the 64-byte swizzle cover all 32 banks) and applies the three filter rows to them
 //   (12 broadcast LDS.128 of weights) for 576 FMAs: 8 FMAs per shared-memory instruction.
 // The layer's weights are staged once per CTA as [chunk][output][tap][16].
-// Small images (flow4..flow6: 8..48 tiles on 148 SMs) split the channel chunks over several CTAs per tile that
+// Small images (flow4..flow6: 8..48 tiles on 132 SMs) split the channel chunks over several CTAs per tile that
 // add their parts with atomics into a zeroed output, as narrow_fwd_kernel does.
 #include "tc_common.cuh"
 

@@ -1,5 +1,5 @@
-// tc_common.cuh -- PTX wrappers (mbarrier, TMA, tcgen05 / tensor memory) and the tensor-map encoder
-// shared by the tensor-core kernels (tc_conv.cu: forward / input gradient, tc_wgrad.cu: weight gradient).
+// tc_common.cuh -- PTX wrappers (mbarrier, TMA, wgmma) and the tensor-map encoder shared by the tensor-core
+// kernels (tc_conv.cu: forward / input gradient, tc_wgrad.cu: weight gradient).
 #pragma once
 #include <cuda.h>
 
@@ -8,17 +8,15 @@
 namespace unflow {
 namespace tc {
 
-constexpr int BM = 128;          // UMMA M
+constexpr int BM = 128;          // rows of a tile: two consumer warpgroups of 64 rows (the wgmma M)
 constexpr int BK = 32;           // fp32 elements per K block = 128 bytes = one swizzle row
-// K blocks accumulated inside the tensor core before the fp32 register add (default of the "tc_chunk" option).
-// Measured on the FlowNetC layers (tools/tc_conv_check.py --chunk-test, error = max |y - y_f64| / max |y_f64|):
-//   4: 1.0e-6   8: 1.8e-6 (-2.5 % time)   16: 3.6e-6 (-3.7 %)   32: 7.1e-6 (-4.3 %)   all of K: 6.8e-9 * K
+// K blocks accumulated by wgmma in one register accumulator before it is added, with round to nearest, to a
+// second fp32 register accumulator (default of the "tc_chunk" option).  A tensor-core accumulation adds with
+// truncation, an error that grows linearly with K; cutting K into chunks bounds it (tc_conv.cu, "Accuracy").
 constexpr int CHUNK = 8;
 constexpr int A_BYTES = BM * BK * 4;   // 16 KB
-extern int g_a_in_tmem;                // tc_conv.cu: A operand of the MMAs in tensor memory (1) or shared memory (0)
 extern long long *g_dbg;               // tc_conv.cu: role-timer buffer (unflow_tc_conv_debug)
-extern int g_chunk;                    // tc_conv.cu: K blocks accumulated in tensor memory between register adds (default CHUNK)
-extern int g_pair;                     // tc_conv.cu: CTA pairs (cta_group::2): 0 never, 1 where the model says so, 2 wherever possible
+extern int g_chunk;                    // tc_conv.cu: K blocks per wgmma accumulation between register adds (default CHUNK)
 
 // ------------------------------------------------------------------------------------------
 // PTX helpers
@@ -43,11 +41,8 @@ __device__ __forceinline__ void mbar_wait(unsigned bar, unsigned parity) {
         : "=r"(done) : "r"(bar), "r"(parity) : "memory");
   } while (!done);
 }
-// One lane of a fully converged warp (elect.sync).  The MMA issuer runs its loop with ALL lanes converged and
-// issues tcgen05.mma / tcgen05.commit under this predicate: ptxas then emits the uniform-datapath instruction
-// once.  Under a plain `if (lane == 0)` it cannot prove that the region is entered by one thread only and wraps
-// EVERY UTCHMMA in an elect-and-branch loop -- the role timers (tools/tc_conv_check.py --roles) showed the issuing
-// thread busy 87 % of the time at ~100 clocks per MMA where the tensor core needs 64.
+// One lane of a fully converged warp (elect.sync): the TMA producer runs its loop with all lanes converged and
+// issues under this predicate.
 __device__ __forceinline__ bool elect_one() {
   unsigned pred = 0;
   asm volatile("{\n .reg .pred p;\n elect.sync _|p, 0xFFFFFFFF;\n selp.u32 %0, 1, 0, p;\n}\n" : "=r"(pred));
@@ -70,127 +65,83 @@ __device__ __forceinline__ void tma_3d(unsigned dst, const CUtensorMap *map, uns
 __device__ __forceinline__ void fence_proxy_async() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
+// barrier over `count` threads (whole warps) with hardware barrier `id` (0 is __syncthreads)
+__device__ __forceinline__ void named_bar_sync(int id, int count) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
+}
 
-// K-major operand tile, 128-byte swizzle: rows of 128 B, 8-row atoms of 1024 B (SBO), descriptor
-// version 1 (sm_100), layout type 2 = SWIZZLE_128B.  (cute::UMMA::SmemDescriptor bit layout.)
-__device__ __forceinline__ unsigned long long umma_desc_k128(unsigned saddr) {
-  return (unsigned long long)((saddr >> 4) & 0x3FFFu) | (1ull << 16) | (64ull << 32) | (1ull << 46) |
-         (2ull << 61);
-}
-// D[tmem] (+)= A[smem] * B[smem]^T, tf32 inputs, fp32 accumulate
-__device__ __forceinline__ void umma_tf32(unsigned d_tmem, unsigned long long adesc, unsigned long long bdesc,
-                                          unsigned idesc, unsigned accumulate) {
-  asm volatile(
-      "{\n .reg .pred p;\n setp.ne.b32 p, %4, 0;\n"
-      " tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n}\n"
-      ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
-// same, A operand from TENSOR MEMORY (lane = row of A, one 32-bit column per K element)
-__device__ __forceinline__ void umma_tf32_ts(unsigned d_tmem, unsigned a_tmem, unsigned long long bdesc,
-                                             unsigned idesc, unsigned accumulate) {
-  asm volatile(
-      "{\n .reg .pred p;\n setp.ne.b32 p, %4, 0;\n"
-      " tcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], %2, %3, p;\n}\n"
-      ::"r"(d_tmem), "r"(a_tmem), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
-// ---- CTA pairs (cta_group::2): two CTAs of a cluster on the two SMs of a TPC run ONE MMA of M = 256: each
-// supplies its own 128 rows of A (tensor memory) and HALF of the B tile (shared memory), the leader issues ----
-__device__ __forceinline__ unsigned cluster_ctarank() {
-  unsigned r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {       // every thread of every CTA of the cluster
-  asm volatile("barrier.cluster.arrive.release.aligned;\n barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// arrive on the barrier that sits at the same shared-memory offset in CTA `cta` of the cluster.  Plain arrive
-// (release at CTA scope): what the leader consumes after it -- tensor-memory stores fenced with
-// tcgen05.fence::before_thread_sync, TMA data whose own barrier this thread has waited on, shared-memory writes
-// behind fence.proxy.async -- is complete when the arrive is sent; `.release.cluster` would put a GPU-scope
-// MEMBAR in front of every arrive (measured: 1900 instead of 770 clk per K block).
-__device__ __forceinline__ void mbar_arrive_cta(unsigned bar, unsigned cta) {
-  unsigned r;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(bar), "r"(cta));
-  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(r) : "memory");
-}
-__device__ __forceinline__ void mbar_wait_cluster(unsigned bar, unsigned parity) {     // pairs with mbar_arrive_cta
-  mbar_wait(bar, parity);
-}
-__device__ __forceinline__ void umma_tf32_ts_pair(unsigned d_tmem, unsigned a_tmem, unsigned long long bdesc,
-                                                  unsigned idesc, unsigned accumulate) {
-  asm volatile(
-      "{\n .reg .pred p;\n setp.ne.b32 p, %4, 0;\n"
-      " tcgen05.mma.cta_group::2.kind::tf32 [%0], [%1], %2, %3, p;\n}\n"
-      ::"r"(d_tmem), "r"(a_tmem), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
-// arrives (once the MMAs issued so far have completed) on the barrier at this offset in BOTH CTAs of the pair
-__device__ __forceinline__ void umma_commit_pair(unsigned bar) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-      ::"r"(bar), "h"((unsigned short)3) : "memory");
-}
-__device__ __forceinline__ void tmem_st32(unsigned taddr, const unsigned (&r)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,"
-      "%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32};"
-      ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]),
-        "r"(r[8]), "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]),
-        "r"(r[16]), "r"(r[17]), "r"(r[18]), "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]),
-        "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]), "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31])
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit(unsigned bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(unsigned taddr, unsigned (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
-      "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-        "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-        "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr) : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_ld16(unsigned taddr, unsigned (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr) : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
 __device__ __forceinline__ float tf32_rna(float x) {
   unsigned u;
   asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(u) : "f"(x));
   return __uint_as_float(u);
 }
-
 // The same rounding (to nearest, ties away from zero) on the integer pipes without cvt's NaN / Inf handling:
-// 2 instead of 4 instructions per element in the converter warps (activations and gradients are finite).
+// 2 instead of 4 instructions per element in the split (activations and gradients are finite).
 __device__ __forceinline__ float tf32_rna_fast(float x) {
   return __uint_as_float((__float_as_uint(x) + 0x1000u) & 0xFFFFE000u);
 }
-
-// MN-major fp32 / tf32 operand tile: the contraction index runs over ROWS of 128 bytes, 32 consecutive
-// M/N elements per row.  For 4-byte types the tensor core accepts exactly one MN-major shared-memory
-// layout: the 128-byte swizzle with 32-BYTE atoms (byte-address bits [5,7) ^= bits [7,9); TMA writes it
-// with CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B; descriptor layout type 1, cute::UMMA
-// SWIZZLE_128B_BASE32B, canonical form ((T,8,m),(4,k)):((1,T,LBO),(8T,SBO))): 4-row groups of 512 B
-// along K (SBO), 32-element groups along M/N `lbo_bytes` apart (LBO).
-__device__ __forceinline__ unsigned long long umma_desc_mn128(unsigned saddr, unsigned lbo_bytes) {
-  return (unsigned long long)((saddr >> 4) & 0x3FFFu) | ((unsigned long long)((lbo_bytes >> 4) & 0x3FFFu) << 16) |
-         (32ull << 32) | (1ull << 46) | (1ull << 61);
+__device__ __forceinline__ float4 tf32_hi4(float4 v) {
+  return make_float4(tf32_rna_fast(v.x), tf32_rna_fast(v.y), tf32_rna_fast(v.z), tf32_rna_fast(v.w));
 }
+__device__ __forceinline__ float4 sub4(float4 a, float4 b) { return make_float4(a.x - b.x, a.y - b.y, a.z - b.z, a.w - b.w); }
+
 __device__ __forceinline__ void red_add_f32(float *addr, float v) {
   asm volatile("red.global.add.f32 [%0], %1;" ::"l"(addr), "f"(v) : "memory");
 }
+
+// ---- wgmma (sm_90a warpgroup MMA) ----------------------------------------------------------------
+// K-major operand tile in the 128-byte swizzle (what TMA writes with CU_TENSOR_MAP_SWIZZLE_128B): rows of
+// 128 B = 32 tf32, 16-byte chunk j of row r stored at chunk j ^ (r & 7), 8-row atoms of 1024 B (stride byte
+// offset), layout type 1 = SWIZZLE_128B.  The tile must start 1024-byte aligned; one K step of 8 tf32 is
+// +32 bytes on the start address (+2 in the descriptor's 16-byte units).
+__device__ __forceinline__ unsigned long long wgmma_desc_k128(unsigned saddr) {
+  return (unsigned long long)((saddr >> 4) & 0x3FFFu) | (1ull << 16) | (64ull << 32) | (1ull << 62);
+}
+// byte offset of element (row r, k) in such a tile
+__device__ __forceinline__ unsigned sw128_offset(int r, int k) {
+  return (unsigned)(r * 128 + ((((k >> 2) ^ (r & 7)) & 7) << 4) + ((k & 3) << 2));
+}
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving reads / writes of the accumulator registers across a wgmma fence or wait
+template <int R>
+__device__ __forceinline__ void fence_regs(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+// D[64 x N] (+)= A[64 x 8] * B[N x 8]^T, tf32 inputs from shared memory (K-major descriptors), fp32 accumulators
+// in registers.  Thread t of the warpgroup holds rows 16 * (t / 32) + (t % 32) / 4 (+ 8) and, in d[4j .. 4j + 3],
+// columns 8j + 2 (t % 4) (+ 1): d[4j + 2h + e] = D[row + 8h][8j + 2 (t % 4) + e].
+template <int N> struct Wgmma;
+template <> struct Wgmma<32> {
+  static __device__ __forceinline__ void mma(float (&d)[16], unsigned long long da, unsigned long long db, int scale_d) {
+    asm volatile(
+        "{\n .reg .pred p;\n setp.ne.b32 p, %18, 0;\n"
+        " wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1;\n}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "l"(da), "l"(db), "r"(scale_d));
+  }
+};
+template <> struct Wgmma<64> {
+  static __device__ __forceinline__ void mma(float (&d)[32], unsigned long long da, unsigned long long db, int scale_d) {
+    asm volatile(
+        "{\n .reg .pred p;\n setp.ne.b32 p, %34, 0;\n"
+        " wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1;\n}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(da), "l"(db), "r"(scale_d));
+  }
+};
+template <> struct Wgmma<128> {
+  static __device__ __forceinline__ void mma(float (&d)[64], unsigned long long da, unsigned long long db, int scale_d) {
+    asm volatile(
+        "{\n .reg .pred p;\n setp.ne.b32 p, %66, 0;\n"
+        " wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1;\n}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(da), "l"(db), "r"(scale_d));
+  }
+};
 
 // ---- host: tensor maps --------------------------------------------------------------------------
 typedef CUresult (*EncodeTiledFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *,
@@ -213,6 +164,7 @@ inline EncodeTiledFn encode_fn() {
 inline int encode(CUtensorMap *m, const float *basep, int rank, const cuuint64_t *dims,
                   const cuuint64_t *strides_bytes, const cuuint32_t *box, const cuuint32_t *estr,
                   CUtensorMapSwizzle swizzle = CU_TENSOR_MAP_SWIZZLE_128B) {
+  if (bind_primary_context()) return UNFLOW_ECUDA;
   EncodeTiledFn fn = encode_fn();
   if (!fn) { set_error("cuTensorMapEncodeTiled entry point not available"); return UNFLOW_ECUDA; }
   CUresult r = fn(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, (cuuint32_t)rank, (void *)basep, dims, strides_bytes, box,

@@ -1,6 +1,6 @@
-// tc_conv.cu -- the conv / deconv stacks of FlowNet on the 5th-generation tensor cores:
-// a tcgen05 implicit GEMM with the 3xTF32 operand split done inside the kernel (activations: into tensor
-// memory; weights: hi / lo planes made once per step).
+// tc_conv.cu -- the conv / deconv stacks of FlowNet on the Hopper tensor cores: a wgmma implicit GEMM with
+// the 3xTF32 operand split done inside the kernel (activations: in shared memory, per K block; weights:
+// hi / lo planes made once per step).
 //
 // Replaces the library convolutions behind slim.conv2d / slim.conv2d_transpose
 // (reference src/e2eflow/core/flownet.py:166-233, _flownet_upconv :89-155) for the forward pass
@@ -18,35 +18,28 @@
 // GEMM view per tile: M = 128 output positions (a TW x TH x TN box of one class), N = BN output
 // channels, K = taps x Cin walked in blocks of 32 channels (one 128-byte swizzle row of fp32).
 //
-// Pipeline (one CTA per SM -- or a cluster of two CTAs on the two SMs of a TPC, see Cfg -- persistent over tiles,
-// warp-specialised; the issuing warps run converged and one elect.sync lane issues, see tc_common.cuh):
-//   warp 0     TMA producer: per K block one 4-D box of the ACTIVATIONS as they lie in HBM (fp32,
-//              NHWC, any channel pitch -- e.g. a channel slice of a concat buffer; image borders,
-//              the TF SAME padding and the channel tail are TMA zero fill, stride 2 is the tensor
-//              map's element stride) plus the hi and lo planes of the weights.
-//   warps 4-7  split the activation tile, thread = tile row: hi = tf32(x), lo = x - hi, both stored to TENSOR
-//              MEMORY (tcgen05.st), the MMAs' A operand.  (Template AT = false keeps the first version: the
-//              split written back to shared memory, A and B both read from there -- bound by shared-memory
-//              bandwidth, profiles/r2_ncu_tc_conv.md.)
-//   warp 1     issues tcgen05.mma kind::tf32, three per K step:
-//              lo*hi' + hi*lo' + hi*hi' accumulate in fp32 in TENSOR MEMORY (double-buffered).
-//   warps 8-15 epilogue: the K loop is cut into CHUNKS of 8 K blocks (tc_common.cuh: CHUNK); the tensor core accumulates one
-//              chunk in tensor memory, these warps read it back (tcgen05.ld) and add it to fp32
-//              REGISTER accumulators with round-to-nearest while the next chunk is being multiplied
-//              into the other TMEM buffer (see "Accuracy"); after the last chunk: bias + leaky ReLU
-//              (or += for gradient accumulation) -> float4 stores straight into the destination
-//              (which may be a channel slice of a concat buffer, with stride 2 for the transposed
-//              classes).  Two warps share a TMEM lane quarter, each owns half of the BN columns.
+// Pipeline (one CTA per SM, persistent over work items, warp-specialised, 3 warpgroups):
+//   warp 0           TMA producer: per K block one 4-D box of the ACTIVATIONS as they lie in HBM (fp32,
+//                    NHWC, any channel pitch -- e.g. a channel slice of a concat buffer; image borders,
+//                    the TF SAME padding and the channel tail are TMA zero fill, stride 2 is the tensor
+//                    map's element stride) plus the hi and lo planes of the weights, into a ring of stages.
+//   warpgroups 1, 2  consumers, 64 tile rows each: split their rows of the activation tile in shared memory
+//                    (hi = tf32(x) in place, lo = x - hi beside it), then issue wgmma m64nBNk8 kind tf32,
+//                    three per K step: lo*hi' + hi*lo' + hi*hi', fp32 accumulators in registers.  The stage
+//                    is released when the next K block's MMAs have been issued and this one's have completed.
+//                    The K loop is cut into CHUNKS of 8 K blocks (tc_common.cuh: CHUNK): every chunk starts a
+//                    fresh wgmma accumulator that is then added to a second fp32 register accumulator with
+//                    round to nearest (see "Accuracy"); after the last chunk: bias + leaky ReLU (or += for
+//                    gradient accumulation) -> stores straight into the destination (which may be a channel
+//                    slice of a concat buffer, with stride 2 for the transposed classes).
 // The activations are read from HBM once, as fp32; no [hi,hi,lo] operand copies exist, no layout
-// conversion, no separate bias / activation pass (round 1 spent 30 % of the step on those).
+// conversion, no separate bias / activation pass.
 //
 // Accuracy: hi carries 11 significant bits, lo the next 11; the dropped lo*lo' term and the
 // truncation of lo are ~2^-22 relative.  What limits a long tensor-core accumulation is not the
 // split but the accumulator itself: the MMA adds with truncation, a bias of a fraction of an ulp
-// per instruction that grows LINEARLY with K (measured on B200, this kernel with one accumulation
-// over all of K and cuDNN's TF32 kernels alike: max error / max|y| = 6.8e-9 * K, i.e. 6e-5 at
-// K = 9216 where an fp32 FMA loop has 2e-5; profiles/r2_tc_conv.md).  Cutting K into chunks of
-// 256 and summing the chunks in fp32 registers (round to nearest) leaves 1.8e-6.
+// per instruction that grows LINEARLY with K.  Summing chunks of 256 K elements in fp32 registers
+// (round to nearest) bounds it.
 #include <algorithm>
 
 #include "tc_common.cuh"
@@ -55,7 +48,7 @@ namespace unflow {
 namespace tc {
 
 constexpr int MAX_TAPS = 64;
-constexpr int NTHREADS = 512;    // 16 warps, see the role table above
+constexpr int NTHREADS = 384;    // warpgroup 0: TMA producer (warp 0); warpgroups 1-2: consumers
 
 struct Tap {
   short dx, dy;
@@ -75,97 +68,55 @@ struct ConvParams {
   const float *bias;          // [Cout] or nullptr
   float slope;                // leaky-ReLU slope when act != 0
   int act, accumulate;
-  int chunk;                  // K blocks accumulated in tensor memory between two register adds (g_chunk)
+  int chunk;                  // K blocks per wgmma accumulation between two register adds (g_chunk)
   long long *dbg;             // role timers of CTA 0 (unflow_tc_conv_debug), or nullptr
   int pair_px;                // two output-parity classes (px = 0, 1) of a narrow transposed layer share one tile, see
                               // pair_px_plan()
   int ksplit;                 // > 1: the K loop of a tile is cut into ksplit work items whose partial sums meet in the
                               // (zeroed) output through red.global.add; bias / activation run as a separate pass
-  int b_mn;                   // weight planes given as [tap][contraction][rows] (the planes of the layer's OTHER direction):
-                              // B tiles are MN-major (32-row x 32-column boxes, 32-byte-atom swizzle) instead of K-major
   int class_start[5];
   short class_px[4], class_py[4];
   Tap taps[MAX_TAPS];
 };
 
-// AT = true (default): the split activation tile (hi, lo) goes to TENSOR MEMORY and the MMAs read their A
-// operand from there.  ncu on the shared-memory variant (profiles/r2_ncu_tc_conv.md) shows the kernel
-// bound by shared-memory bandwidth: LSU wavefronts (the split: read 16 KB, write 32 KB per K block) 48 % +
-// tensor-core operand reads (12 MMAs x (4 KB A + 4 KB B)) 53 % of the peak, tensor pipe 52 % busy.  With
-// A in TMEM the split writes nothing to shared memory and the MMAs fetch only B from it: 64 KB instead of
-// 144 KB of shared-memory traffic per K block, and a stage shrinks from 64 to 48 KB (4 stages).
-// What limits the AT kernel is the SM's ingress from L2: 48 KB per K block (16 KB activations + 32 KB
-// hi / lo weight planes) at ~43 B/clk -- ncu: 10.4 TB/s chip-wide, the fabric limit -- for 768 clk of MMA
-// work.  Two ways to cut it were tried on B200 and measured slower / equal, and removed again: (1) fetching
-// the fp32 weights once and splitting them in the kernel too (32 KB per K block): 756 us instead of 680 us
-// for conv3_1 forward with the two spare warps doing the split, 680 instead of 617 us with the work spread
-// over all six converter warps -- the extra shared-memory round trip of the weight tile costs more than the
-// saved ingress; (2) TMA multicast of the
-// weight tiles to CTA pairs (the ingress per SM is unchanged, and L2 already merges the concurrent reads:
-// 679 us vs 680 us).  A cta_group::2 MMA (each SM holds half of B) is the remaining lever.
-//
-// CG = 2 (CTA pair, cta_group::2): the two CTAs of a cluster take two M tiles of the SAME column block; each
-// loads its own activation box and HALF of the weight tile (BN/2 rows of the hi and lo planes), the leader's
-// MMAs (M = 256) read both halves.  Per SM and K block that is 16 + 16 KB of ingress instead of 16 + 32 KB
-// (BN = 128) -- below the 768 clk of MMA work -- and 16 + 8 instead of 16 + 16 KB for BN = 64.
-template <int BN, bool AT, int CG = 1>
+// Stage: [A raw -> hi after the split] [A lo] [B hi] [B lo].  Each 1024-byte aligned (128-byte swizzle atoms).
+template <int BN>
 struct Cfg {
-  static_assert(CG == 1 || (CG == 2 && AT && BN >= 64), "CTA pairs: tensor-memory A operand, BN 64 / 128");
-  static constexpr int B_BYTES = BN / CG * BK * 4;               // this CTA's part of one weight plane
-  static constexpr int STAGE_BYTES = (AT ? 1 : 2) * A_BYTES + 2 * B_BYTES;
-  static constexpr int B_OFF = (AT ? 1 : 2) * A_BYTES;          // offset of the weight planes inside a stage
-  // Two rings: STAGES shared-memory stages (TMA -> converter / MMA) and, with the A operand in tensor memory,
-  // ASLOTS operand slots there (converter -> MMA).  Tensor memory has room for (512 - 2 BN) / 64 slots only (4 at
-  // BN = 128), shared memory for more stages of a CTA pair's 32 KB: the TMA ring is the one that has to cover the
-  // L2 latency, so it runs deeper than the slot ring (role timers with 4 = 4: every role idle ~50 % at 830-900
-  // clocks per K block; tools/tc_conv_check.py --roles).
-  static constexpr int MAX_SLOTS = (512 - 2 * BN) / (2 * BK);
+  static constexpr int B_BYTES = BN * BK * 4;
+  static constexpr int STAGE_BYTES = 2 * A_BYTES + 2 * B_BYTES;
+  static constexpr int B_OFF = 2 * A_BYTES;
   static constexpr int STAGES = (200 * 1024 / STAGE_BYTES) < 8 ? (200 * 1024 / STAGE_BYTES) : 8;
-  static constexpr int ASLOTS = !AT ? STAGES : (STAGES < MAX_SLOTS ? STAGES : MAX_SLOTS);
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*alignment slack*/ + 512 /*barriers*/;
-  static constexpr int ACC_COLS = 2 * BN;                        // two accumulator buffers
-  static constexpr int A_COLS = AT ? ASLOTS * 2 * BK : 0;        // per slot: 32 columns hi + 32 columns lo
-  static constexpr int NEED = ACC_COLS + A_COLS;
-  static constexpr int TMEM_COLS = NEED <= 32 ? 32 : NEED <= 64 ? 64 : NEED <= 128 ? 128 : NEED <= 256 ? 256 : 512;
-  static_assert(NEED <= 512, "tensor memory has 512 columns");
+  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*alignment slack*/ + 256 /*barriers*/;
+  static_assert(STAGES >= 2, "at least two stages");
 };
 
 struct TileCoord {
   int cls, n0, iy0, ix0, nb;
 };
-// Tile order, fastest first: column block, output-parity class, M tile (CG = 2: PAIR of M tiles; CTA `rank`
-// takes M tile 2 * pair + rank; past the last M tile the box lies behind the last image: TMA zero fill, no
-// stores).  The classes of a transposed layer all read the same input box: next to each other in the schedule
-// they run at the same time on neighbouring SMs and share it in L2 -- with the class outermost every class
-// swept the whole input again (ncu on deconv2 / the input gradient of conv2: 4x the input in DRAM reads, 82 %
-// L2 read hit rate, the TMA ring starved).
-template <int CG>
-__device__ __forceinline__ TileCoord decode_tile(const ConvParams &p, int tile, int rank) {
+// Tile order, fastest first: column block, output-parity class, M tile.  The classes of a transposed layer all
+// read the same input box: next to each other in the schedule they run at the same time on neighbouring SMs and
+// share it in L2 (with the class outermost every class would sweep the whole input again).
+__device__ __forceinline__ TileCoord decode_tile(const ConvParams &p, int tile) {
   TileCoord t;
   t.nb = tile % p.n_blocks; tile /= p.n_blocks;
   t.cls = tile % p.n_classes; tile /= p.n_classes;
-  if (CG == 2) {
-    tile = 2 * tile + rank;
-    if (tile >= p.tiles_n * p.tiles_y * p.tiles_x) { t.ix0 = t.iy0 = 0; t.n0 = p.tiles_n * p.TN; return t; }
-  }
   t.ix0 = (tile % p.tiles_x) * p.TW; tile /= p.tiles_x;
   t.iy0 = (tile % p.tiles_y) * p.TH; tile /= p.tiles_y;
   t.n0 = tile * p.TN;
   return t;
 }
 
-// Work item = (tile, K slice).  Layers with few tiles (conv6 / conv6_1 of the step: 32 pair tiles for 74 SM pairs,
-// 288 K blocks each) cut the K loop of a tile into p.ksplit slices that run at the same time on different CTAs
-// (adjacent in the schedule: the slice index is the fastest).
+// Work item = (tile, K slice).  Layers with few tiles and long K loops (conv6 / conv6_1) cut the K loop of a tile
+// into p.ksplit slices that run at the same time on different CTAs (adjacent in the schedule: the slice index is
+// the fastest).
 struct Work {
   TileCoord t;
   int it0, iters;       // first K block (tap * kblocks + channel block) and count of this item
 };
-template <int CG>
-__device__ __forceinline__ Work decode_work(const ConvParams &p, int w, int rank) {
+__device__ __forceinline__ Work decode_work(const ConvParams &p, int w) {
   Work k;
   const int tile = w / p.ksplit, ks = w - tile * p.ksplit;
-  k.t = decode_tile<CG>(p, tile, rank);
+  k.t = decode_tile(p, tile);
   const int total = (p.class_start[k.t.cls + 1] - p.class_start[k.t.cls]) * p.kblocks;
   const int per = (total + p.ksplit - 1) / p.ksplit;
   k.it0 = ks * per;
@@ -177,346 +128,181 @@ __device__ __forceinline__ Work decode_work(const ConvParams &p, int w, int rank
 // ------------------------------------------------------------------------------------------
 // The kernel
 // ------------------------------------------------------------------------------------------
-template <int BN, bool AT, int CG>
+template <int BN>
 __global__ void __launch_bounds__(NTHREADS, 1)
 tc_conv_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapBhi,
                const __grid_constant__ CUtensorMap mapBlo, const __grid_constant__ ConvParams p) {
-  using C = Cfg<BN, AT, CG>;
+  using C = Cfg<BN>;
+  constexpr int R = BN / 2;              // accumulator registers per thread (64 x BN per warpgroup)
   extern __shared__ unsigned char smem_raw[];
   const unsigned base = (s32(smem_raw) + 1023u) & ~1023u;          // 128B swizzle atoms need 1024 B alignment
   unsigned char *gbase = smem_raw + (base - s32(smem_raw));
-  // stage layout: [A raw (= hi after the split when !AT)] [A lo, only when !AT] [B hi] [B lo]
   const unsigned bars = base + C::STAGES * C::STAGE_BYTES;
-  constexpr int NB0 = 2 * C::STAGES + 2 * C::ASLOTS;               // barriers before the accumulator ones
-  auto full_raw = [&](int s) { return bars + 8u * s; };               // stage s landed (TMA)
-  auto empty = [&](int s) { return bars + 8u * (C::STAGES + s); };    // stage s consumed (MMAs done)
-  auto full_cvt = [&](int a) { return bars + 8u * (2 * C::STAGES + a); };               // operand slot a written
-  auto a_empty = [&](int a) { return bars + 8u * (2 * C::STAGES + C::ASLOTS + a); };    // operand slot a consumed
-  auto tmem_full = [&](int a) { return bars + 8u * (NB0 + a); };
-  auto tmem_empty = [&](int a) { return bars + 8u * (NB0 + 2 + a); };
-  const unsigned tmem_slot = bars + 8u * (NB0 + 4);
-  volatile unsigned *tmem_slot_ptr = (volatile unsigned *)(gbase + C::STAGES * C::STAGE_BYTES + 8 * (NB0 + 4));
+  auto full = [&](int s) { return bars + 8u * s; };                   // stage s landed (TMA)
+  auto empty = [&](int s) { return bars + 8u * (C::STAGES + s); };    // stage s consumed (MMAs of both consumers done)
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int m_tiles = p.tiles_n * p.tiles_y * p.tiles_x;
-  const int total_tiles = p.n_classes * (CG == 2 ? (m_tiles + 1) / 2 : m_tiles) * p.n_blocks * p.ksplit;   // work items
-  // CG = 2: the two CTAs of a cluster walk the same tile sequence; rank 0 (the leader) issues the MMAs and owns
-  // the barriers both CTAs arrive on (full_cvt, tmem_empty); full_raw / empty / tmem_full stay per CTA
-  const int rank = CG == 2 ? (int)cluster_ctarank() : 0;
-  const int first_tile = CG == 2 ? (int)(blockIdx.x >> 1) : (int)blockIdx.x;
-  const int tile_step = CG == 2 ? (int)(gridDim.x >> 1) : (int)gridDim.x;
+  const int total_items = p.n_classes * m_tiles * p.n_blocks * p.ksplit;
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < C::STAGES; ++s) {
-      mbar_init(full_raw(s), 1);
-      mbar_init(empty(s), 1);
-    }
-    for (int a = 0; a < C::ASLOTS; ++a) {
-      mbar_init(full_cvt(a), 4 * CG);
-      mbar_init(a_empty(a), 1);
-    }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(tmem_full(a), 1);
-      mbar_init(tmem_empty(a), 8 * CG);
+      mbar_init(full(s), 1);
+      mbar_init(empty(s), 8);          // one arrive per consumer warp
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&mapA) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&mapBhi) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&mapBlo) : "memory");
   }
-  if (warp == 2) {
-    if (CG == 2) {       // one warp of EACH CTA of the pair, same warp id, same destination offset
-      asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tmem_slot),
-                   "r"((unsigned)C::TMEM_COLS) : "memory");
-      asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-    } else {
-      asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tmem_slot),
-                   "r"((unsigned)C::TMEM_COLS) : "memory");
-      asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-  }
-  tc_fence_before();
-  if (CG == 2) cluster_sync_all(); else __syncthreads();     // pair: the peer's barriers are initialised too
-  tc_fence_after();
-  const unsigned tmem_base = *tmem_slot_ptr;
+  __syncthreads();
 
   if (warp == 0) {
     // ===================== TMA producer (whole warp converged, one elected lane issues) =====================
-    {
-      int s = 0;
-      unsigned ph = 0;
-      long long t_wait = 0, t_all = clock64();          // role timers: cycles blocked on the barrier / in total
-      const unsigned a_box_bytes = (unsigned)(p.TW * p.TH * p.TN) * BK * 4u;
-      for (int tile = first_tile; tile < total_tiles; tile += tile_step) {
-        const Work wk = decode_work<CG>(p, tile, rank);
-        const TileCoord t = wk.t;
-        const int x0 = p.s_in_x * t.ix0, y0 = p.s_in_y * t.iy0;
-        // pair: this CTA's half of the weight rows (pair_px: rows 0.. of its own class's tap)
-        const int brow = p.pair_px ? 0 : t.nb * BN + rank * (BN / CG);
-        int ti = p.class_start[t.cls] + wk.it0 / p.kblocks, kc = wk.it0 % p.kblocks;
-        {
-          for (int it = 0; it < wk.iters; ++it) {
-            Tap tap = p.taps[ti];
-            if (p.pair_px) {         // rank 0 loads the weights of class px = 0, rank 1 those of px = 1; no tap: zero fill
-              const int wi = rank ? tap.widx2 : tap.widx;
-              tap.widx = wi < 0 ? (1 << 20) : wi;
-            }
-            { const long long t0 = clock64(); mbar_wait(empty(s), ph ^ 1u); t_wait += clock64() - t0; }
-            const unsigned st = base + s * C::STAGE_BYTES;
-            if (elect_one()) {
-              mbar_expect_tx(full_raw(s), a_box_bytes + 2u * C::B_BYTES);
-              tma_4d(st, &mapA, full_raw(s), kc * BK, x0 + tap.dx, y0 + tap.dy, t.n0);
-              if (p.b_mn) {        // 32 contraction rows x 32 output columns per box, BN / CG / 32 boxes per plane
-#pragma unroll
-                for (int j = 0; j < BN / CG / 32; ++j) {
-                  tma_3d(st + C::B_OFF + j * 4096, &mapBhi, full_raw(s), brow + 32 * j, kc * BK, tap.widx);
-                  tma_3d(st + C::B_OFF + C::B_BYTES + j * 4096, &mapBlo, full_raw(s), brow + 32 * j, kc * BK, tap.widx);
-                }
-              } else {
-                tma_3d(st + C::B_OFF, &mapBhi, full_raw(s), kc * BK, brow, tap.widx);
-                tma_3d(st + C::B_OFF + C::B_BYTES, &mapBlo, full_raw(s), kc * BK, brow, tap.widx);
-              }
-            }
-            __syncwarp();
-            if (++s == C::STAGES) { s = 0; ph ^= 1u; }
-            if (++kc == p.kblocks) { kc = 0; ++ti; }
-          }
-        }
-      }
-      if (p.dbg && blockIdx.x == 0 && lane == 0) { p.dbg[0] = t_wait; p.dbg[1] = clock64() - t_all; }
-    }
-  } else if (warp == 1) {
-    // ===================== MMA issuer (whole warp converged, one elected lane issues) =====================
-    if (rank == 0) {
-      // instruction descriptor: D fp32, A/B tf32, both K-major, N = BN, M = 128 (256 over a CTA pair)
-      const unsigned idesc = (1u << 4) | (2u << 7) | (2u << 10) | (p.b_mn ? (1u << 16) : 0u) |
-                             ((unsigned)(BN >> 3) << 17) | ((unsigned)((CG * BM) >> 4) << 24);
-      const unsigned long long kstep = p.b_mn ? 64ull : 2ull;    // 8 contraction elements: 8 rows of 128 B / 32 bytes
-      int s = 0, acc = 0, sl = 0;
-      unsigned ph = 0, aph = 0, slph = 0;
-      long long t_wait_acc = 0, t_wait_ops = 0, t_all = clock64();
-      for (int tile = first_tile; tile < total_tiles; tile += tile_step) {
-        const int iters = decode_work<CG>(p, tile, rank).iters;
-        for (int it = 0; it < iters; ++it) {
-          const int in_chunk = it % p.chunk;
-          if (in_chunk == 0) {               // a fresh TMEM accumulator for every chunk of K
-            const long long t0 = clock64();
-            if (CG == 2) mbar_wait_cluster(tmem_empty(acc), aph ^ 1u); else mbar_wait(tmem_empty(acc), aph ^ 1u);
-            t_wait_acc += clock64() - t0;
-            tc_fence_after();
-          }
-          const long long t1 = clock64();
-          const unsigned d = tmem_base + (unsigned)(acc * BN);
-          if (CG == 2) {
-            // the converter warps of BOTH CTAs arrive here after their own TMA barrier: activations split and
-            // both halves of the weight tile landed
-            mbar_wait_cluster(full_cvt(sl), slph);
+    int s = 0;
+    unsigned ph = 0;
+    long long t_wait = 0, t_all = clock64();          // role timers: cycles blocked on the barrier / in total
+    const unsigned a_box_bytes = (unsigned)(p.TW * p.TH * p.TN) * BK * 4u;
+    for (int item = blockIdx.x; item < total_items; item += gridDim.x) {
+      const Work wk = decode_work(p, item);
+      const TileCoord t = wk.t;
+      const int x0 = p.s_in_x * t.ix0, y0 = p.s_in_y * t.iy0;
+      int ti = p.class_start[t.cls] + wk.it0 / p.kblocks, kc = wk.it0 % p.kblocks;
+      for (int it = 0; it < wk.iters; ++it) {
+        const Tap tap = p.taps[ti];
+        { const long long t0 = clock64(); mbar_wait(empty(s), ph ^ 1u); t_wait += clock64() - t0; }
+        const unsigned st = base + s * C::STAGE_BYTES;
+        if (elect_one()) {
+          mbar_expect_tx(full(s), a_box_bytes + 2u * C::B_BYTES);
+          tma_4d(st, &mapA, full(s), kc * BK, x0 + tap.dx, y0 + tap.dy, t.n0);
+          if (p.pair_px) {      // rows [0, BN/2): the weights of class px = 0, [BN/2, BN): px = 1; no tap: zero fill
+            const int w0 = tap.widx < 0 ? (1 << 20) : tap.widx, w1 = tap.widx2 < 0 ? (1 << 20) : tap.widx2;
+            tma_3d(st + C::B_OFF, &mapBhi, full(s), kc * BK, 0, w0);
+            tma_3d(st + C::B_OFF + C::B_BYTES / 2, &mapBhi, full(s), kc * BK, 0, w1);
+            tma_3d(st + C::B_OFF + C::B_BYTES, &mapBlo, full(s), kc * BK, 0, w0);
+            tma_3d(st + C::B_OFF + C::B_BYTES + C::B_BYTES / 2, &mapBlo, full(s), kc * BK, 0, w1);
           } else {
-            mbar_wait(full_raw(s), ph);        // weights landed (TMA)
-            mbar_wait(full_cvt(sl), slph);     // activations split (converter warps)
+            tma_3d(st + C::B_OFF, &mapBhi, full(s), kc * BK, t.nb * BN, tap.widx);
+            tma_3d(st + C::B_OFF + C::B_BYTES, &mapBlo, full(s), kc * BK, t.nb * BN, tap.widx);
           }
-          t_wait_ops += clock64() - t1;
-          tc_fence_after();
-          const unsigned st = base + s * C::STAGE_BYTES;
-          const unsigned long long b_hi = p.b_mn ? umma_desc_mn128(st + C::B_OFF, 4096) : umma_desc_k128(st + C::B_OFF);
-          const unsigned long long b_lo = p.b_mn ? umma_desc_mn128(st + C::B_OFF + C::B_BYTES, 4096)
-                                                 : umma_desc_k128(st + C::B_OFF + C::B_BYTES);
-          if (elect_one()) {
-          if (CG == 2) {
-            const unsigned ta_hi = tmem_base + (unsigned)(C::ACC_COLS + sl * 2 * BK), ta_lo = ta_hi + BK;
-#pragma unroll
-            for (int k = 0; k < BK / 8; ++k) {
-              const unsigned long long adv = kstep * (unsigned long long)k;
-              umma_tf32_ts_pair(d, ta_lo + 8 * k, b_hi + adv, idesc, (in_chunk | k) != 0);
-              umma_tf32_ts_pair(d, ta_hi + 8 * k, b_lo + adv, idesc, 1u);
-              umma_tf32_ts_pair(d, ta_hi + 8 * k, b_hi + adv, idesc, 1u);
-            }
-          } else if (AT) {
-            const unsigned ta_hi = tmem_base + (unsigned)(C::ACC_COLS + sl * 2 * BK), ta_lo = ta_hi + BK;
-#pragma unroll
-            for (int k = 0; k < BK / 8; ++k) {          // A: 8 TMEM columns per K step; B: +32 bytes
-              const unsigned long long adv = kstep * (unsigned long long)k;
-              umma_tf32_ts(d, ta_lo + 8 * k, b_hi + adv, idesc, (in_chunk | k) != 0);
-              umma_tf32_ts(d, ta_hi + 8 * k, b_lo + adv, idesc, 1u);
-              umma_tf32_ts(d, ta_hi + 8 * k, b_hi + adv, idesc, 1u);
-            }
-          } else {
-            const unsigned long long a_hi = umma_desc_k128(st), a_lo = umma_desc_k128(st + A_BYTES);
-#pragma unroll
-            for (int k = 0; k < BK / 8; ++k) {          // UMMA K = 8 tf32 = 32 bytes: +2 in 16-byte units
-              const unsigned long long adv = kstep * (unsigned long long)k, adva = (unsigned long long)(2 * k);
-              umma_tf32(d, a_lo + adva, b_hi + adv, idesc, (in_chunk | k) != 0);
-              umma_tf32(d, a_hi + adva, b_lo + adv, idesc, 1u);
-              umma_tf32(d, a_hi + adva, b_hi + adv, idesc, 1u);
-            }
-          }
-          // frees the stage and the operand slot when these MMAs have read them (pair: in both CTAs)
-          if (CG == 2) umma_commit_pair(empty(s)); else umma_commit(empty(s));
-          if (AT) { if (CG == 2) umma_commit_pair(a_empty(sl)); else umma_commit(a_empty(sl)); }
-          if (in_chunk == p.chunk - 1 || it == iters - 1) {
-            // chunk complete -> epilogue warps (of both CTAs) add it to their registers
-            if (CG == 2) umma_commit_pair(tmem_full(acc)); else umma_commit(tmem_full(acc));
-          }
-          }     // elect_one
-          __syncwarp();
-          if (++s == C::STAGES) { s = 0; ph ^= 1u; }
-          if (++sl == C::ASLOTS) { sl = 0; slph ^= 1u; }
-          if (in_chunk == p.chunk - 1 || it == iters - 1) {
-            if (++acc == 2) { acc = 0; aph ^= 1u; }
-          }
-        }
-      }
-      if (p.dbg && blockIdx.x == 0 && lane == 0) { p.dbg[2] = t_wait_acc; p.dbg[3] = t_wait_ops; p.dbg[4] = clock64() - t_all; }
-    }
-  } else if (warp >= 4 && warp < 8) {
-    // ===================== activation split =====================
-    const int tid = threadIdx.x - 128;
-    int s = 0, sl = 0;
-    unsigned ph = 0, slph = 0;
-    long long t_wait = 0, t_all = clock64();
-    for (int tile = first_tile; tile < total_tiles; tile += tile_step) {
-      const int iters = decode_work<CG>(p, tile, rank).iters;
-      for (int it = 0; it < iters; ++it) {
-        { const long long t0 = clock64(); mbar_wait(full_raw(s), ph); t_wait += clock64() - t0; }
-        if (AT) { mbar_wait(a_empty(sl), slph ^ 1u); tc_fence_after(); }   // the MMAs that read this operand slot last are done
-        if (AT) {
-          // thread = tile row: read the row's 32 channels (8 x 16 bytes; the 128-byte swizzle stores logical
-          // chunk j of row r at chunk j ^ (r & 7) -- a quarter warp hits all 32 banks), split, and store
-          // hi / lo into this stage's tensor-memory columns (lane = row, one column per channel)
-          const float4 *rowp = reinterpret_cast<const float4 *>(gbase + s * C::STAGE_BYTES + tid * 128);
-          unsigned hi[BK], lo[BK];
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            const float4 v = rowp[j ^ (tid & 7)];
-            const float x4[4] = {v.x, v.y, v.z, v.w};
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-              const float h = tf32_rna_fast(x4[e]);
-              hi[4 * j + e] = __float_as_uint(h);
-              lo[4 * j + e] = __float_as_uint(x4[e] - h);
-            }
-          }
-          const unsigned ta = tmem_base + ((unsigned)((warp & 3) * 32) << 16) + (unsigned)(C::ACC_COLS + sl * 2 * BK);
-          tmem_st32(ta, hi);
-          tmem_st32(ta + BK, lo);
-          asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-          tc_fence_before();
-        } else {
-          float4 *a = reinterpret_cast<float4 *>(gbase + s * C::STAGE_BYTES);
-          float4 *l = reinterpret_cast<float4 *>(gbase + s * C::STAGE_BYTES + A_BYTES);
-#pragma unroll
-          for (int j = 0; j < A_BYTES / 16 / 128; ++j) {
-            const int i = tid + 128 * j;
-            const float4 v = a[i];
-            float4 h, r;
-            h.x = tf32_rna_fast(v.x); h.y = tf32_rna_fast(v.y); h.z = tf32_rna_fast(v.z); h.w = tf32_rna_fast(v.w);
-            r.x = v.x - h.x; r.y = v.y - h.y; r.z = v.z - h.z; r.w = v.w - h.w;
-            a[i] = h;
-            l[i] = r;
-          }
-          fence_proxy_async();                 // generic-proxy writes -> visible to the tensor core
         }
         __syncwarp();
-        if (lane == 0) {
-          if (CG == 2) mbar_arrive_cta(full_cvt(sl), 0); else mbar_arrive(full_cvt(sl));
-        }
         if (++s == C::STAGES) { s = 0; ph ^= 1u; }
-        if (++sl == C::ASLOTS) { sl = 0; slph ^= 1u; }
+        if (++kc == p.kblocks) { kc = 0; ++ti; }
       }
     }
-    if (p.dbg && blockIdx.x == 0 && threadIdx.x == 128) { p.dbg[5] = t_wait; p.dbg[6] = clock64() - t_all; }
-  } else if (warp >= 8) {
-    // ===================== epilogue: fp32 register accumulation over the K chunks =====================
-    constexpr int COLS = BN / 2;             // columns per thread: warps 8-11 take the low half, 12-15 the high half
-    const int q = warp & 3;                  // the TMEM lane quarter this warp may read (warp id % 4)
-    const int half = (warp - 8) >> 2;
-    const int row = q * 32 + lane;
+    if (p.dbg && blockIdx.x == 0 && lane == 0) { p.dbg[0] = t_wait; p.dbg[1] = clock64() - t_all; }
+  } else if (warp >= 4) {
+    // ===================== consumers: split, wgmma, epilogue =====================
+    const int cw = (warp >> 2) - 1;                  // consumer warpgroup: tile rows [64 cw, 64 cw + 64)
+    const int ct = threadIdx.x - 128 * (cw + 1);     // thread within the warpgroup
+    const int row0 = 64 * cw + 16 * (ct >> 5) + (lane >> 2);     // this thread's accumulator rows: row0, row0 + 8
+    const int col0 = 2 * (lane & 3);
     const int per_img = p.TW * p.TH;
-    const int tn = row / per_img, rem = row - tn * per_img;
-    const int ty = rem / p.TW, tx = rem - ty * p.TW;
-    int acc = 0;
-    unsigned aph = 0;
+    int s = 0;
+    unsigned ph = 0;
     long long t_wait = 0, t_all = clock64();
-    for (int tile = first_tile; tile < total_tiles; tile += tile_step) {
-      const Work wk = decode_work<CG>(p, tile, rank);
+    float sum[R], acc[R];
+    for (int item = blockIdx.x; item < total_items; item += gridDim.x) {
+      const Work wk = decode_work(p, item);
       const TileCoord t = wk.t;
       const int iters = wk.iters;
-      const int chunks = (iters + p.chunk - 1) / p.chunk;
-      float sum[COLS];
 #pragma unroll
-      for (int c = 0; c < COLS; ++c) sum[c] = 0.f;
-      for (int ck = 0; ck < chunks; ++ck) {
-        { const long long t0 = clock64(); mbar_wait(tmem_full(acc), aph); t_wait += clock64() - t0; }
-        tc_fence_after();
-        const unsigned taddr = tmem_base + ((unsigned)(q * 32) << 16) + (unsigned)(acc * BN + half * COLS);
+      for (int c = 0; c < R; ++c) sum[c] = 0.f;
+      int pending = -1;                              // stage whose MMAs may still be running
+      for (int it = 0; it < iters; ++it) {
+        const int in_chunk = it % p.chunk;
+        const bool chunk_end = in_chunk == p.chunk - 1 || it == iters - 1;
+        { const long long t0 = clock64(); mbar_wait(full(s), ph); t_wait += clock64() - t0; }
+        // split this warpgroup's 64 rows (8 KB): the elementwise split keeps the swizzled positions
+        {
+          float4 *a = reinterpret_cast<float4 *>(gbase + s * C::STAGE_BYTES + cw * (A_BYTES / 2));
+          float4 *l = reinterpret_cast<float4 *>(gbase + s * C::STAGE_BYTES + A_BYTES + cw * (A_BYTES / 2));
 #pragma unroll
-        for (int c0 = 0; c0 < COLS; c0 += 16) {
-          unsigned r[16];
-          tmem_ld16(taddr + (unsigned)c0, r);
-#pragma unroll
-          for (int e = 0; e < 16; ++e) sum[c0 + e] += __uint_as_float(r[e]);
+          for (int j = 0; j < A_BYTES / 2 / 16 / 128; ++j) {
+            const int i = ct + 128 * j;
+            const float4 v = a[i], h = tf32_hi4(v);
+            a[i] = h;
+            l[i] = sub4(v, h);
+          }
         }
-        tc_fence_before();
+        fence_proxy_async();                         // generic-proxy writes -> visible to the tensor core
+        named_bar_sync(1 + cw, 128);
+        const unsigned st = base + s * C::STAGE_BYTES;
+        const unsigned long long a_hi = wgmma_desc_k128(st + cw * (A_BYTES / 2));
+        const unsigned long long a_lo = wgmma_desc_k128(st + A_BYTES + cw * (A_BYTES / 2));
+        const unsigned long long b_hi = wgmma_desc_k128(st + C::B_OFF), b_lo = wgmma_desc_k128(st + C::B_OFF + C::B_BYTES);
+        fence_regs(acc);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < BK / 8; ++k) {           // K step = 8 tf32 = 32 bytes: +2 in 16-byte units
+          const unsigned long long adv = (unsigned long long)(2 * k);
+          Wgmma<BN>::mma(acc, a_lo + adv, b_hi + adv, (in_chunk | k) != 0);
+          Wgmma<BN>::mma(acc, a_hi + adv, b_lo + adv, 1);
+          Wgmma<BN>::mma(acc, a_hi + adv, b_hi + adv, 1);
+        }
+        wgmma_commit();
+        if (chunk_end) wgmma_wait<0>(); else wgmma_wait<1>();
+        fence_regs(acc);
+        // the MMAs of the previous K block (and at a chunk end of this one) have completed: free their stages
         __syncwarp();
-        if (lane == 0) {
-          if (CG == 2) mbar_arrive_cta(tmem_empty(acc), 0); else mbar_arrive(tmem_empty(acc));
+        if (pending >= 0 && lane == 0) mbar_arrive(empty(pending));
+        pending = s;
+        if (chunk_end) {
+          if (lane == 0) mbar_arrive(empty(s));
+          pending = -1;
+#pragma unroll
+          for (int c = 0; c < R; ++c) sum[c] += acc[c];
         }
-        if (++acc == 2) { acc = 0; aph ^= 1u; }
+        if (++s == C::STAGES) { s = 0; ph ^= 1u; }
       }
-      const int n = t.n0 + tn, iy = t.iy0 + ty, ix = t.ix0 + tx;
-      const bool valid = tn < p.TN && n < p.N && iy < p.Hit && ix < p.Wit;
-      // pair_px: the two column halves of the tile are the two px classes of the same (<= 64) output channels
-      const int oy = p.s_out * iy + p.class_py[t.cls], ox = p.s_out * ix + (p.pair_px ? half : p.class_px[t.cls]);
-      const int cbase = p.pair_px ? 0 : t.nb * BN + half * COLS;          // first output channel of this thread
-      if (valid && cbase < p.Cout && p.ksplit > 1) {
-        // K slice: add the raw partial sums (the launcher zeroed the output unless it accumulates anyway)
-        float *dst = p.out + (((long long)n * p.Hout + oy) * p.Wout + ox) * p.out_pitch + cbase;
-        if (chunks > 0) {
+      // ---- epilogue: rows row0 and row0 + 8, columns 8j + col0 (+1) ----
 #pragma unroll
-          for (int c = 0; c < COLS; ++c)
-            if (cbase + c < p.Cout) red_add_f32(dst + c, sum[c]);
-        }
-      } else if (valid && cbase < p.Cout) {
-        float *dst = p.out + (((long long)n * p.Hout + oy) * p.Wout + ox) * p.out_pitch + cbase;
+      for (int h = 0; h < 2; ++h) {
+        const int row = row0 + 8 * h;
+        const int tn = row / per_img, rem = row - tn * per_img;
+        const int ty = rem / p.TW, tx = rem - ty * p.TW;
+        const int n = t.n0 + tn, iy = t.iy0 + ty, ix = t.ix0 + tx;
+        if (!(tn < p.TN && n < p.N && iy < p.Hit && ix < p.Wit)) continue;
+        const int oy = p.s_out * iy + p.class_py[t.cls];
+        float *const orow = p.out + ((long long)n * p.Hout + oy) * p.Wout * p.out_pitch;
 #pragma unroll
-        for (int j = 0; j < COLS / 4; ++j) {
-          const int c = cbase + 4 * j;
-          float v[4] = {sum[4 * j], sum[4 * j + 1], sum[4 * j + 2], sum[4 * j + 3]};
-          if (c + 4 <= p.Cout) {
-            if (p.bias) {                          // scalar loads: a bias is a view into the flat variable
-#pragma unroll                                     // buffer at any 4-byte offset
-              for (int e = 0; e < 4; ++e) v[e] += __ldg(p.bias + c + e);
+        for (int j = 0; j < BN / 8; ++j) {
+          const int col = 8 * j + col0;
+          // pair_px: the two column halves of the tile are the two px classes of the same (<= 64) output channels
+          const int half = p.pair_px && col >= BN / 2 ? 1 : 0;
+          const int c = p.pair_px ? col - half * (BN / 2) : t.nb * BN + col;
+          const int ox = p.s_out * ix + (p.pair_px ? half : p.class_px[t.cls]);
+          if (c >= p.Cout) continue;
+          float *dst = orow + (long long)ox * p.out_pitch + c;
+          float v0 = sum[4 * j + 2 * h], v1 = sum[4 * j + 2 * h + 1];
+          const bool two = c + 1 < p.Cout;
+          if (p.ksplit > 1) {        // K slice: add the raw partial sums (the launcher zeroed the output unless it accumulates anyway)
+            if (iters > 0) {
+              red_add_f32(dst, v0);
+              if (two) red_add_f32(dst + 1, v1);
             }
-            if (p.act) {
-#pragma unroll
-              for (int e = 0; e < 4; ++e) v[e] = v[e] > 0.f ? v[e] : p.slope * v[e];
-            }
-            float4 *o = reinterpret_cast<float4 *>(dst) + j;
-            if (p.accumulate) {
-              const float4 old = *o;
-              v[0] += old.x; v[1] += old.y; v[2] += old.z; v[3] += old.w;
-            }
-            *o = make_float4(v[0], v[1], v[2], v[3]);
-          } else if (c < p.Cout) {                 // channel tail (C_out not a multiple of 4)
-            for (int e = 0; e < 4 && c + e < p.Cout; ++e) {
-              float u = v[e] + (p.bias ? __ldg(p.bias + c + e) : 0.f);
-              if (p.act) u = u > 0.f ? u : p.slope * u;
-              float *o = dst + 4 * j + e;
-              *o = p.accumulate ? *o + u : u;
-            }
+            continue;
+          }
+          if (p.bias) {              // scalar loads: a bias is a view into the flat variable buffer at any 4-byte offset
+            v0 += __ldg(p.bias + c);
+            if (two) v1 += __ldg(p.bias + c + 1);
+          }
+          if (p.act) {
+            v0 = v0 > 0.f ? v0 : p.slope * v0;
+            v1 = v1 > 0.f ? v1 : p.slope * v1;
+          }
+          if (two) {                 // c is even and the pitch a multiple of 4: 8-byte aligned
+            float2 *o = reinterpret_cast<float2 *>(dst);
+            if (p.accumulate) { const float2 old = *o; v0 += old.x; v1 += old.y; }
+            *o = make_float2(v0, v1);
+          } else {                   // channel tail
+            *dst = p.accumulate ? *dst + v0 : v0;
           }
         }
       }
     }
-    if (p.dbg && blockIdx.x == 0 && threadIdx.x == 256) { p.dbg[7] = t_wait; p.dbg[8] = clock64() - t_all; }
-  }
-  tc_fence_before();
-  if (CG == 2) cluster_sync_all(); else __syncthreads();      // pair: the peer may still be reading / being read
-  if (warp == 2) {
-    if (CG == 2)
-      asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((unsigned)C::TMEM_COLS) : "memory");
-    else
-      asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((unsigned)C::TMEM_COLS) : "memory");
+    if (p.dbg && blockIdx.x == 0 && threadIdx.x == 128) { p.dbg[2] = t_wait; p.dbg[3] = clock64() - t_all; }
   }
 }
 
@@ -559,104 +345,55 @@ wsplit_kernel(const float *__restrict__ w, float *__restrict__ hi, float *__rest
 // ------------------------------------------------------------------------------------------
 static int floordiv(int a, int b) { return (a >= 0) ? a / b : -((-a + b - 1) / b); }
 
-int g_a_in_tmem = 1;     // unflow_set_int_option("tc_a_tmem"): 1 = A operand in tensor memory (default), 0 = in shared memory
-int g_chunk = CHUNK;     // unflow_set_int_option("tc_chunk"): K blocks per tensor-memory accumulation
+int g_chunk = CHUNK;     // unflow_set_int_option("tc_chunk"): K blocks per wgmma accumulation
 int g_pair_px = 1;       // unflow_set_int_option("tc_pair_px"): 1 = narrow transposed layers compute two parity classes per tile
 int g_ksplit = 1;        // unflow_set_int_option("tc_ksplit"): 1 = layers with few tiles cut their K loops into slices, 0 = never
 long long *g_dbg = nullptr;   // unflow_tc_conv_debug: device buffer of 16 long longs for the role timers of CTA 0
-int g_pair = 1;          // unflow_set_int_option("tc_pair"): 0 = single CTAs only, 1 = CTA pairs where the model below says so, 2 = wherever possible
 
-template <int BN, bool AT, int CG>
-static int launch_v(const CUtensorMap &mA, const CUtensorMap &mBh, const CUtensorMap &mBl, const ConvParams &p,
-                    int total_tiles, cudaStream_t stream) {
-  using C = Cfg<BN, AT, CG>;
+template <int BN>
+static int launch(const CUtensorMap &mA, const CUtensorMap &mBh, const CUtensorMap &mBl, const ConvParams &p,
+                  cudaStream_t stream) {
+  using C = Cfg<BN>;
   static bool attr_set = false;
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(tc_conv_kernel<BN, AT, CG>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES);
+    cudaError_t e = cudaFuncSetAttribute(tc_conv_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES);
     if (e != cudaSuccess) { set_error("tc_conv: cannot opt in to %d bytes of shared memory: %s", C::SMEM_BYTES, cudaGetErrorString(e)); return UNFLOW_ECUDA; }
     attr_set = true;
   }
-  if (CG == 2) {                       // clusters of two CTAs: the pair sits on the two SMs of one TPC
-    const int pairs = total_tiles < kNumSMs / 2 ? total_tiles : kNumSMs / 2;
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(2 * pairs); cfg.blockDim = dim3(NTHREADS); cfg.dynamicSmemBytes = C::SMEM_BYTES; cfg.stream = stream;
-    cudaLaunchAttribute at[1];
-    at[0].id = cudaLaunchAttributeClusterDimension;
-    at[0].val.clusterDim.x = 2; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
-    cfg.attrs = at; cfg.numAttrs = 1;
-    cudaError_t e = cudaLaunchKernelEx(&cfg, tc_conv_kernel<BN, AT, CG>, mA, mBh, mBl, p);
-    if (e != cudaSuccess) { set_error("tc_conv: cluster launch failed: %s", cudaGetErrorString(e)); return UNFLOW_ECUDA; }
-  } else {
-    const int grid = total_tiles < kNumSMs ? total_tiles : kNumSMs;
-    tc_conv_kernel<BN, AT, CG><<<grid, NTHREADS, C::SMEM_BYTES, stream>>>(mA, mBh, mBl, p);
-  }
+  const long long total = (long long)p.n_classes * p.tiles_n * p.tiles_y * p.tiles_x * p.n_blocks * p.ksplit;
+  const int grid = total < kNumSMs ? (int)total : kNumSMs;
+  tc_conv_kernel<BN><<<grid, NTHREADS, C::SMEM_BYTES, stream>>>(mA, mBh, mBl, p);
   count_launch();
   return check_launch("tc_conv_kernel");
 }
 
-// Single CTAs or pairs?  Time model per K block and CTA, in clocks: the MMAs (768 at BN = 128) against the SM's
-// ingress from L2 (~43 B/clk) of the activation box plus this CTA's share of the two weight planes; times the
-// number of waves the tiles need on 148 SMs / 74 pairs.
-inline int pick_cta_group(const ConvParams &p, int BN) {
-  if (p.pair_px) return 2;
-  if (!g_a_in_tmem || g_pair == 0 || BN < 64) return 1;
-  const long long m_tiles = (long long)p.tiles_n * p.tiles_y * p.tiles_x;
-  if (m_tiles < 2) return 1;
-  if (g_pair == 2) return 2;
-  const double mma = 768.0 * BN / 128.0;
-  const double t1 = std::max(mma, (16384.0 + 2.0 * BN * 128.0) / 43.0), t2 = std::max(mma, (16384.0 + BN * 128.0) / 43.0);
-  const long long tiles1 = p.n_classes * m_tiles * p.n_blocks, tiles2 = p.n_classes * ((m_tiles + 1) / 2) * p.n_blocks;
-  const double w1 = (double)((tiles1 + kNumSMs - 1) / kNumSMs) * t1, w2 = (double)((tiles2 + kNumSMs / 2 - 1) / (kNumSMs / 2)) * t2;
-  return w2 < w1 ? 2 : 1;
-}
-
-template <int BN>
-static int launch(const CUtensorMap &mA, const CUtensorMap &mBh, const CUtensorMap &mBl, const ConvParams &p,
-                  int cta_group, cudaStream_t stream) {
-  const int m_tiles = p.tiles_n * p.tiles_y * p.tiles_x;
-  const int total = p.n_classes * (cta_group == 2 ? (m_tiles + 1) / 2 : m_tiles) * p.n_blocks * p.ksplit;
-  if constexpr (BN >= 64) {
-    if (cta_group == 2) return launch_v<BN, true, 2>(mA, mBh, mBl, p, total, stream);
-  }
-  return g_a_in_tmem ? launch_v<BN, true, 1>(mA, mBh, mBl, p, total, stream)
-                     : launch_v<BN, false, 1>(mA, mBh, mBl, p, total, stream);
-}
-
-// K slices for a layer with few tiles and long K loops (work items <= half of the SMs / SM pairs): how many
-inline int choose_ksplit(const ConvParams &p, int BN) {
+// K slices for a layer with few tiles and long K loops (work items <= half of the SMs): how many
+inline int choose_ksplit(const ConvParams &p) {
   if (!g_ksplit) return 1;
-  const int cg = pick_cta_group(p, BN);
-  const long long m_tiles = (long long)p.tiles_n * p.tiles_y * p.tiles_x;
-  const long long items = p.n_classes * (cg == 2 ? (m_tiles + 1) / 2 : m_tiles) * p.n_blocks;
-  const long long slots = cg == 2 ? kNumSMs / 2 : kNumSMs;
-  if (2 * items > slots) return 1;
+  const long long items = (long long)p.n_classes * p.tiles_n * p.tiles_y * p.tiles_x * p.n_blocks;
+  if (2 * items > kNumSMs) return 1;
   int min_iters = 1 << 30;
   for (int c = 0; c < p.n_classes; ++c) min_iters = std::min(min_iters, (p.class_start[c + 1] - p.class_start[c]) * p.kblocks);
-  const long long ks = std::min<long long>(std::min<long long>(slots / items, 4), std::max(1, min_iters / (4 * p.chunk)));
+  const long long ks = std::min<long long>(std::min<long long>(kNumSMs / items, 4), std::max(1, min_iters / (4 * p.chunk)));
   return ks < 1 ? 1 : (int)ks;
 }
 
-// tile -> kernel: encodes the two weight-plane maps (box = this CTA's rows) and launches
+// tile -> kernel: encodes the two weight-plane maps (box = BN rows, or BN / 2 for pair_px) and launches
 static int launch_bn(int BN, const CUtensorMap &mA, const float *w_hi, const float *w_lo, const cuuint64_t *wdims,
                      const cuuint64_t *wstrides, const ConvParams &p, cudaStream_t stream) {
-  const int cg = pick_cta_group(p, BN);
   CUtensorMap mBh, mBl;
-  cuuint32_t box[3] = {(cuuint32_t)BK, (cuuint32_t)(BN / cg), 1};
-  if (p.b_mn) { box[0] = 32; box[1] = (cuuint32_t)BK; }      // planes [tap][contraction][rows]: 32 rows x 32 contraction
+  cuuint32_t box[3] = {(cuuint32_t)BK, (cuuint32_t)(p.pair_px ? BN / 2 : BN), 1};
   cuuint32_t estr[3] = {1, 1, 1};
-  const CUtensorMapSwizzle swz = p.b_mn ? CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B : CU_TENSOR_MAP_SWIZZLE_128B;
-  int rc = encode(&mBh, w_hi, 3, wdims, wstrides, box, estr, swz);
+  int rc = encode(&mBh, w_hi, 3, wdims, wstrides, box, estr);
   if (rc) return rc;
-  rc = encode(&mBl, w_lo, 3, wdims, wstrides, box, estr, swz);
+  rc = encode(&mBl, w_lo, 3, wdims, wstrides, box, estr);
   if (rc) return rc;
-  if (BN == 128) return launch<128>(mA, mBh, mBl, p, cg, stream);
-  if (BN == 64) return launch<64>(mA, mBh, mBl, p, cg, stream);
-  return launch<32>(mA, mBh, mBl, p, cg, stream);
+  if (BN == 128) return launch<128>(mA, mBh, mBl, p, stream);
+  if (BN == 64) return launch<64>(mA, mBh, mBl, p, stream);
+  return launch<32>(mA, mBh, mBl, p, stream);
 }
 
 }  // namespace tc
-int set_tc_a_tmem(int v) { if (v != 0 && v != 1) return 0; tc::g_a_in_tmem = v; return 1; }
-int set_tc_pair(int v) { if (v < 0 || v > 2) return 0; tc::g_pair = v; return 1; }
 int set_tc_chunk(int v) { if (v < 1 || v > 64) return 0; tc::g_chunk = v; return 1; }
 int set_tc_ksplit(int v) { if (v != 0 && v != 1) return 0; tc::g_ksplit = v; return 1; }
 int set_tc_pair_px(int v) { if (v != 0 && v != 1) return 0; tc::g_pair_px = v; return 1; }
@@ -737,15 +474,14 @@ static int make_plan(tc::ConvParams &p, int &BN, int N, int Hin, int Win, int Ci
   return UNFLOW_OK;
 }
 
-// Narrow transposed layers (33..64 output channels: deconv2, the input gradient of conv2): the MMA costs the same
-// for N = 64 as for N = 128 (profiles/r2_mma_probe.md), so a 64-wide tile wastes half of the tensor core.  The
-// two output-parity classes px = 0 / 1 of a row class py read overlapping input offsets (k4 s2: dx {0,-1} and
-// {+1,0}; 5x5 s2: {0,-1} and {+1,0,-1}): ONE 128-wide tile computes both -- columns [0,64) = the channels of
-// px = 0, [64,128) = those of px = 1 -- over the union of the offsets; where only one class has a tap for an
-// offset the other half of the weight tile is TMA zero fill.  CTA pairs only: rank r loads the weights of class
-// px = r (its half of B).  K blocks per channel block over all classes: k4 s2 12 instead of 16, 5x5 s2 15 instead of 25.
+// Narrow transposed layers (33..64 output channels: deconv2, the input gradient of conv2): the two output-parity
+// classes px = 0 / 1 of a row class py read overlapping input offsets (k4 s2: dx {0,-1} and {+1,0}; 5x5 s2: {0,-1}
+// and {+1,0,-1}): ONE 128-wide tile computes both -- columns [0,64) = the channels of px = 0, [64,128) = those of
+// px = 1 -- over the union of the offsets; where only one class has a tap for an offset that half of the weight
+// tile is TMA zero fill.  Each activation box is loaded and split once for both classes, and a channel block
+// walks fewer K blocks over all classes: k4 s2 12 instead of 16, 5x5 s2 15 instead of 25.
 static bool pair_px_plan(tc::ConvParams &p, int &BN, int mode, int stride, int Cout) {
-  if (!tc::g_pair_px || !tc::g_pair || !tc::g_a_in_tmem || mode != 1 || stride != 2 || p.n_classes != 4) return false;
+  if (!tc::g_pair_px || mode != 1 || stride != 2 || p.n_classes != 4) return false;
   if (Cout <= 32 || Cout > 64 || (long long)p.tiles_n * p.tiles_y * p.tiles_x < 2) return false;
   tc::Tap taps[tc::MAX_TAPS];
   int start[3], nt = 0;
@@ -779,9 +515,8 @@ static bool pair_px_plan(tc::ConvParams &p, int &BN, int mode, int stride, int C
 }
 
 // Debug hook: role timers.  `buf` = device memory for 16 long longs (or nullptr to switch off); every following
-// tc_conv launch makes CTA 0 write, in clocks: [0] TMA producer blocked on a free stage, [1] its total; [2] MMA
-// issuer blocked on a free accumulator, [3] on the operands of a K block, [4] its total; [5] converter warp 4
-// blocked on the TMA data, [6] its total; [7] epilogue warp 8 blocked on a finished chunk, [8] its total.
+// tc_conv launch makes CTA 0 write, in clocks: [0] TMA producer blocked on a free stage, [1] its total; [2] the
+// first consumer thread blocked on the TMA data, [3] its total.
 extern "C" int unflow_tc_conv_debug(long long *buf) { tc::g_dbg = buf; return UNFLOW_OK; }
 
 // Debug / test hook: the plan as integers --
@@ -820,8 +555,6 @@ extern "C" int unflow_tc_conv(const float *x, int N, int Hin, int Win, int Cin, 
                               long long y_pitch, const float *bias, float slope, int act, int accumulate,
                               int mode, int stride, int kh, int kw, int pad_t, int pad_l, void *stream) {
   UNFLOW_REQUIRE(x && w_hi && w_lo && y, "tc_conv: null pointer");
-  const int planes_t = (mode >> 1) & 1;          // bit 1: the planes are [taps][Cin][Cout_p] (see include/unflow.h)
-  mode &= 1;
   UNFLOW_REQUIRE(x_pitch % 4 == 0 && y_pitch % 4 == 0 && x_pitch >= Cin && y_pitch >= Cout,
                  "tc_conv: channel pitches must be multiples of 4 floats");
   UNFLOW_REQUIRE(((uintptr_t)x & 15) == 0 && ((uintptr_t)y & 15) == 0 && ((uintptr_t)w_hi & 15) == 0 &&
@@ -832,11 +565,11 @@ extern "C" int unflow_tc_conv(const float *x, int N, int Hin, int Win, int Cin, 
   if (rc0) return rc0;
   pair_px_plan(p, BN, mode, stride, Cout);
   p.out = y; p.out_pitch = y_pitch;
-  p.bias = bias; p.slope = slope; p.act = act; p.accumulate = accumulate; p.b_mn = planes_t;
+  p.bias = bias; p.slope = slope; p.act = act; p.accumulate = accumulate;
   // K slices (few tiles, long K): partial sums are added into the output, which is zeroed first unless the call
   // accumulates anyway; bias + leaky ReLU then run as unflow_bias_lrelu over the (dense) result
   const bool post = bias && act;
-  if ((!bias && !act) || (post && y_pitch == Cout && Cout % 4 == 0)) p.ksplit = tc::choose_ksplit(p, BN);
+  if ((!bias && !act) || (post && y_pitch == Cout && Cout % 4 == 0)) p.ksplit = tc::choose_ksplit(p);
   if (p.ksplit > 1 && !accumulate) {
     cudaError_t e = cudaMemset2DAsync(y, (size_t)y_pitch * 4, 0, (size_t)Cout * 4, (size_t)N * Hout * Wout, (cudaStream_t)stream);
     if (e != cudaSuccess) { set_error("tc_conv: memset of the output: %s", cudaGetErrorString(e)); return UNFLOW_ECUDA; }
@@ -851,18 +584,10 @@ extern "C" int unflow_tc_conv(const float *x, int N, int Hin, int Win, int Cin, 
     int rc = tc::encode(&mA, x, 4, dims, strides, box, estr);
     if (rc) return rc;
   }
-  int rc;
-  if (planes_t) {
-    const int Cop = (Cout + 3) / 4 * 4;
-    cuuint64_t wdims[3] = {(cuuint64_t)Cout, (cuuint64_t)Cin, (cuuint64_t)(kh * kw)};
-    cuuint64_t wstrides[2] = {(cuuint64_t)Cop * 4, (cuuint64_t)Cop * 4 * Cin};
-    rc = tc::launch_bn(BN, mA, w_hi, w_lo, wdims, wstrides, p, (cudaStream_t)stream);
-  } else {
-    const int Cp = (Cin + 3) / 4 * 4;
-    cuuint64_t wdims[3] = {(cuuint64_t)Cin, (cuuint64_t)Cout, (cuuint64_t)(kh * kw)};
-    cuuint64_t wstrides[2] = {(cuuint64_t)Cp * 4, (cuuint64_t)Cp * 4 * Cout};
-    rc = tc::launch_bn(BN, mA, w_hi, w_lo, wdims, wstrides, p, (cudaStream_t)stream);
-  }
+  const int Cp = (Cin + 3) / 4 * 4;
+  cuuint64_t wdims[3] = {(cuuint64_t)Cin, (cuuint64_t)Cout, (cuuint64_t)(kh * kw)};
+  cuuint64_t wstrides[2] = {(cuuint64_t)Cp * 4, (cuuint64_t)Cp * 4 * Cout};
+  const int rc = tc::launch_bn(BN, mA, w_hi, w_lo, wdims, wstrides, p, (cudaStream_t)stream);
   if (rc || p.ksplit == 1 || !post) return rc;
   return unflow_bias_lrelu(y, bias, (long long)N * Hout * Wout, Cout, slope, stream);
 }

@@ -1,5 +1,5 @@
-// tc_wgrad.cu -- weight gradients of the conv / deconv stacks on the tensor cores (tcgen05,
-// 3xTF32 split of BOTH operands in shared memory, fp32 register accumulation, split-K).
+// tc_wgrad.cu -- weight gradients of the conv / deconv stacks on the Hopper tensor cores (wgmma, 3xTF32
+// split of BOTH operands in shared memory, fp32 register accumulation, split-K).
 //
 // Replaces the library weight-gradient kernels behind tf.gradients of slim.conv2d /
 // slim.conv2d_transpose (reference src/e2eflow/core/flownet.py:166-233, :89-155; train.py:151-152)
@@ -11,26 +11,23 @@
 //   transposed    y = deconv(x, W):   P = x     (rows r = C_in),  G = dL/dy (cols c = C_out), stride 2
 //
 // GEMM view per work item: M = 128 rows of P's channels, N = BN channels of G, K = pixels.  NHWC
-// memory has the channels contiguous and the contraction index (pixels) across rows: G is used as an
-// "MN-major" shared-memory operand -- exactly what a TMA box of 32 pixels x 32 channels (one 128-byte row
-// per pixel, in the 32-byte-atom swizzle the tensor core requires of MN-major tf32 operands) delivers --
-// and P is transposed for free on its way into tensor memory.  No transposed copy of any activation exists.
+// memory has the channels contiguous and the contraction index (pixels) across rows, while wgmma reads tf32
+// operands K-major only: TMA brings boxes of 32 pixels x 32 channels as they lie in memory, and the split into
+// hi / lo writes them TRANSPOSED (row = channel, 32 pixels per 128-byte row, 128-byte swizzle).  No transposed
+// copy of any activation exists in global memory.
 //
 // Work item = (pixel chunk, 128-row block, BN-column block); the BN columns are BN/32 consecutive
-// (tap, 32-channel group) pairs, so a layer with few input channels fills the 128-wide MMA with
-// several taps at once (conv2: 64 channels -> two taps per block).  A chunk is a run of 32-pixel K
-// blocks sized so that the grid has a few waves of items; items of one chunk are adjacent in the
-// schedule, so the chunk's activations are read from HBM once and re-read from L2.
-//   warp 0      TMA: per K block 4 boxes of P (32 px x 32 ch each) and BN/32 boxes of G (element
-//               stride = the conv stride, tap offset in the start coordinate, zero fill outside)
-//   warps 4-7   P tile -> hi / lo in TENSOR MEMORY (lane = channel: the transposing read is free)
-//   warps 2-3, 16-19   G tile: hi = tf32(v) in place, lo = v - hi beside it (shared memory).  20 warps: with 16
-//               (G shared between warps 2-3 and 4-7) the converter warps were busy 85 % of the time and the MMA
-//               issuer waited 40 % for operands; 24 warps leave 80 registers per thread and spill (slower).
-//   warp 1      tcgen05.mma kind::tf32, A from tensor memory, B MN-major from shared memory:
-//               lo*hi + hi*lo + hi*hi per 8-pixel K step
-//   warps 8-15  every 8 K blocks: tcgen05.ld the TMEM accumulator and add it to fp32 registers (see
-//               tc_conv.cu, "Accuracy"); at the end of the item: red.global.add into dW
+// (tap, 32-channel group) pairs, so a layer with few input channels fills the tile with several taps at
+// once (conv2: 64 channels -> two taps per block).  A chunk is a run of 32-pixel K blocks sized so that the
+// grid has a few waves of items; items of one chunk are adjacent in the schedule, so the chunk's
+// activations are read from HBM once and re-read from L2.
+//   warp 0           TMA: per K block 4 boxes of P (32 px x 32 ch each) and BN/32 boxes of G (element
+//                    stride = the conv stride, tap offset in the start coordinate, zero fill outside)
+//   warpgroups 1, 2  each splits + transposes its 64 rows of P and half of the G tile, then (after a barrier
+//                    over both, since both read all of G) issues wgmma m64nBNk8 for its 64 rows:
+//                    lo*hi + hi*lo + hi*hi per 8-pixel K step; every 8 K blocks the wgmma accumulator is
+//                    added to fp32 registers (see tc_conv.cu, "Accuracy"); at the end of the item:
+//                    red.global.add into dW
 // dW is accumulated with fp32 atomics (split-K partial sums from several CTAs): the caller zeroes
 // it; the order of the additions, hence the last bits, vary from run to run.
 #include "tc_common.cuh"
@@ -40,8 +37,7 @@ namespace tcw {
 
 using namespace unflow::tc;
 
-constexpr int NTHREADS = 640;       // 20 warps: 0 TMA, 1 MMA, 2-3 + 16-19 G split, 4-7 P -> tensor memory, 8-15 epilogue
-constexpr int GWARPS = 6;
+constexpr int NTHREADS = 384;       // warpgroup 0: TMA (warp 0); warpgroups 1-2: split + MMA + epilogue
 constexpr int KP = 32;              // pixels per K block
 
 struct WgradParams {
@@ -52,56 +48,36 @@ struct WgradParams {
   int R, C;                         // rows (channels of P) / columns (channels of G) of dW
   int cgroups, vgroups;             // 32-channel groups of G per tap; (tap, group) pairs = "virtual" column groups
   int r_blocks, c_blocks, taps, kw;  // c_blocks: blocks of BN/32 consecutive virtual groups
-  int chunk;                        // K blocks per tensor-memory accumulation (tc::g_chunk)
+  int chunk;                        // K blocks per wgmma accumulation (tc::g_chunk)
   long long *dbg;                   // role timers of CTA 0 (unflow_tc_conv_debug), or nullptr
-  int trunc;                        // experiment: hi = the raw fp32 (the tensor core drops the low 13 bits itself), lo = x - trunc(x)
-  int g_first;                      // float4s of the G tile split by warps 4-7 (after their P tile); warps 2-3 take the rest
   int stride, stride_x, pad_t, pad_l;   // stride_x = 1 in the row-window form (x stride inside the tensor map)
   float *dw;
   long long pitch_r, pitch_t;       // dW[r * pitch_r + t * pitch_t + c]
 };
 
-// The split P tile (the MMA's A operand) lives in TENSOR MEMORY (see tc_conv.cu, Cfg): converter warps read
-// it from a plain (unswizzled) staging tile -- lane = channel, one LDS.32 per pixel, which is also the
-// transpose the K-major TMEM operand needs -- and store hi / lo with tcgen05.st; only G is split in shared
-// memory (hi in place, lo beside it) for the MMAs.
-//
-// CG = 2 (CTA pair, cta_group::2, see tc_conv.cu): the two CTAs take two ROW blocks of the same (chunk, column
-// block) item; each converts its own P tile and loads + splits HALF of the G tile (BN/64 of the 32-channel
-// groups), the leader's MMAs (M = 256) read both halves.  The single-CTA kernel is bound by shared-memory
-// bandwidth -- per K block 32 KB written by TMA, 16 + 16 KB read and 32 KB written by the converter warps, 48 KB
-// read by the MMAs: 144 KB against 128 B/clk x 768 clk -- the pair moves 88 KB per CTA.
-template <int BN, int CG = 1>
+// Stage: [P raw] [G raw] (TMA, unswizzled: per 32-channel group [32 px][32 ch]) and the split, transposed
+// operands [P hi] [P lo] [G hi] [G lo] (K-major, 128-byte swizzle).  Every part is a multiple of 4 KB.
+template <int BN>
 struct Cfg {
-  static_assert(CG == 1 || (CG == 2 && BN == 128), "CTA pairs: BN = 128");
-  static constexpr int B_BYTES = BN / CG * KP * 4;               // this CTA's part of the G tile
-  static constexpr int STAGE_BYTES = A_BYTES + 2 * B_BYTES;
-  static constexpr int B_OFF = A_BYTES;
-  // shared-memory stages (TMA ring) and tensor-memory operand slots for the split P tile (see tc_conv.cu, Cfg)
+  static constexpr int G_BYTES = BN * KP * 4;
+  static constexpr int G_RAW = A_BYTES;
+  static constexpr int A_HI = G_RAW + G_BYTES;
+  static constexpr int A_LO = A_HI + A_BYTES;
+  static constexpr int B_HI = A_LO + A_BYTES;
+  static constexpr int B_LO = B_HI + G_BYTES;
+  static constexpr int STAGE_BYTES = B_LO + G_BYTES;
   static constexpr int STAGES = (200 * 1024 / STAGE_BYTES) < 8 ? (200 * 1024 / STAGE_BYTES) : 8;
-  static constexpr int MAX_SLOTS = (512 - 2 * BN) / (2 * KP);
-  static constexpr int ASLOTS = STAGES < MAX_SLOTS ? STAGES : MAX_SLOTS;
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 + 512;
-  static constexpr int ACC_COLS = 2 * BN;
-  static constexpr int A_COLS = ASLOTS * 2 * KP;
-  static constexpr int NEED = ACC_COLS + A_COLS;
-  static constexpr int TMEM_COLS = NEED <= 32 ? 32 : NEED <= 64 ? 64 : NEED <= 128 ? 128 : NEED <= 256 ? 256 : 512;
-  static_assert(NEED <= 512, "tensor memory has 512 columns");
+  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 + 256;
+  static_assert(STAGES >= 2, "at least two stages");
 };
 
 struct Item {
   int chunk, rb, cb;
 };
-template <int CG>
-__device__ __forceinline__ Item decode_item(const WgradParams &p, int it, int rank) {
+__device__ __forceinline__ Item decode_item(const WgradParams &p, int it) {
   Item w;
   w.cb = it % p.c_blocks; it /= p.c_blocks;
-  if (CG == 2) {                 // pair: row blocks 2i and 2i + 1 (past the last one: rows >= R, zero fill, no stores)
-    const int rp = (p.r_blocks + 1) / 2;
-    w.rb = 2 * (it % rp) + rank; it /= rp;
-  } else {
-    w.rb = it % p.r_blocks; it /= p.r_blocks;
-  }
+  w.rb = it % p.r_blocks; it /= p.r_blocks;
   w.chunk = it;
   return w;
 }
@@ -110,383 +86,184 @@ __device__ __forceinline__ int chunk_len(const WgradParams &p, int chunk) {
   return (k0 + p.kc <= p.n_ptiles) ? p.kc : p.n_ptiles - k0;
 }
 
-template <int BN, int CG>
+// raw [group][32 px][32 ch] tile -> rows [row0, row0 + rows) of the transposed hi / lo tiles, one float4 of
+// 4 pixels per item; consecutive threads take consecutive rows (conflict-free reads and swizzled writes)
+template <int ROWS>
+__device__ __forceinline__ void split_transpose(const float *raw, unsigned char *hi, unsigned char *lo, int row0, int ct) {
+#pragma unroll
+  for (int j = 0; j < ROWS * 8 / 128; ++j) {
+    const int i = ct + 128 * j;
+    const int r = row0 + i % ROWS, c = i / ROWS;
+    const float *src = raw + (r >> 5) * 1024 + (4 * c) * 32 + (r & 31);
+    const float4 v = make_float4(src[0], src[32], src[64], src[96]), h = tf32_hi4(v);
+    const unsigned o = sw128_offset(r, 4 * c);
+    *reinterpret_cast<float4 *>(hi + o) = h;
+    *reinterpret_cast<float4 *>(lo + o) = sub4(v, h);
+  }
+}
+
+template <int BN>
 __global__ void __launch_bounds__(NTHREADS, 1)
 tc_wgrad_kernel(const __grid_constant__ CUtensorMap mapP, const __grid_constant__ CUtensorMap mapG,
                 const __grid_constant__ WgradParams p) {
-  using C = Cfg<BN, CG>;
-  constexpr int GROUPS = BN / 32 / CG;        // 32-channel groups of G this CTA loads and splits
+  using C = Cfg<BN>;
+  constexpr int R = BN / 2;
+  constexpr int GROUPS = BN / 32;
   extern __shared__ unsigned char smem_raw[];
   const unsigned base = (s32(smem_raw) + 1023u) & ~1023u;
   unsigned char *gbase = smem_raw + (base - s32(smem_raw));
-  // stage layout: [P hi (raw)] [P lo] [G hi (raw)] [G lo]; each tile = channel groups of 32 (4096 B each)
   const unsigned bars = base + C::STAGES * C::STAGE_BYTES;
-  auto full_raw = [&](int s) { return bars + 8u * s; };
-  auto full_cvt = [&](int s) { return bars + 8u * (C::STAGES + s); };
-  auto empty = [&](int s) { return bars + 8u * (2 * C::STAGES + s); };
-  constexpr int NB0 = 3 * C::STAGES + C::ASLOTS;
-  auto a_empty = [&](int a) { return bars + 8u * (3 * C::STAGES + a); };     // operand slot a consumed by the MMAs
-  auto tmem_full = [&](int a) { return bars + 8u * (NB0 + a); };
-  auto tmem_empty = [&](int a) { return bars + 8u * (NB0 + 2 + a); };
-  const unsigned tmem_slot = bars + 8u * (NB0 + 4);
-  volatile unsigned *tmem_slot_ptr = (volatile unsigned *)(gbase + C::STAGES * C::STAGE_BYTES + 8 * (NB0 + 4));
+  auto full = [&](int s) { return bars + 8u * s; };
+  auto empty = [&](int s) { return bars + 8u * (C::STAGES + s); };
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int total_items = p.n_chunks * (CG == 2 ? (p.r_blocks + 1) / 2 : p.r_blocks) * p.c_blocks;
-  // CG = 2: both CTAs of the cluster walk the same items; rank 0 issues the MMAs and owns full_cvt / tmem_empty
-  const int rank = CG == 2 ? (int)cluster_ctarank() : 0;
-  const int first_item = CG == 2 ? (int)(blockIdx.x >> 1) : (int)blockIdx.x;
-  const int item_step = CG == 2 ? (int)(gridDim.x >> 1) : (int)gridDim.x;
+  const int total_items = p.n_chunks * p.r_blocks * p.c_blocks;
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < C::STAGES; ++s) {
-      mbar_init(full_raw(s), 1);
-      mbar_init(full_cvt(s), (4 + GWARPS) * CG);   // 4 warps (P -> tensor memory) + 6 warps (G in shared memory), per CTA
-      mbar_init(empty(s), 1);
-    }
-    for (int a = 0; a < C::ASLOTS; ++a) mbar_init(a_empty(a), 1);
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(tmem_full(a), 1);
-      mbar_init(tmem_empty(a), 8 * CG);
+      mbar_init(full(s), 1);
+      mbar_init(empty(s), 8);          // one arrive per consumer warp
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&mapP) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&mapG) : "memory");
   }
-  if (warp == 2) {
-    if (CG == 2) {
-      asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tmem_slot),
-                   "r"((unsigned)C::TMEM_COLS) : "memory");
-      asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-    } else {
-      asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tmem_slot),
-                   "r"((unsigned)C::TMEM_COLS) : "memory");
-      asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-  }
-  tc_fence_before();
-  if (CG == 2) cluster_sync_all(); else __syncthreads();
-  tc_fence_after();
-  const unsigned tmem_base = *tmem_slot_ptr;
+  __syncthreads();
 
   if (warp == 0) {
     // ===================== TMA producer (whole warp converged, one elected lane issues) =====================
-    {
-      int s = 0;
-      unsigned ph = 0;
-      long long t_wait = 0, t_all = clock64();
-      for (int item = first_item; item < total_items; item += item_step) {
-        const Item w = decode_item<CG>(p, item, rank);
-        int gch[GROUPS], gdx[GROUPS], gdy[GROUPS];           // per column group of this CTA: channel, tap offset
-#pragma unroll
-        for (int j = 0; j < GROUPS; ++j) {
-          const int v = w.cb * (BN / 32) + rank * GROUPS + j;
-          if (v < p.vgroups) {
-            const int tap = v / p.cgroups, ky = tap / p.kw;
-            gch[j] = (v - tap * p.cgroups) * 32; gdy[j] = ky - p.pad_t; gdx[j] = tap - ky * p.kw - p.pad_l;
-          } else {
-            gch[j] = p.cgroups * 32; gdx[j] = gdy[j] = 0;    // past the last group: channels >= C, TMA zero fill
-          }
-        }
-        const int k0 = w.chunk * p.kc, klen = chunk_len(p, w.chunk);
-        for (int kb = k0; kb < k0 + klen; ++kb) {
-          int q = kb;
-          const int px = (q % p.tiles_x) * p.TW; q /= p.tiles_x;
-          const int py = (q % p.tiles_y) * p.TH; q /= p.tiles_y;
-          const int pn = q * p.TN;
-          { const long long t0 = clock64(); mbar_wait(empty(s), ph ^ 1u); t_wait += clock64() - t0; }
-          const unsigned st = base + s * C::STAGE_BYTES;
-          if (elect_one()) {
-            mbar_expect_tx(full_raw(s), (unsigned)(A_BYTES + C::B_BYTES));
-#pragma unroll
-            for (int j = 0; j < BM / 32; ++j)       // channels past R are TMA zero fill
-              tma_4d(st + j * 4096, &mapP, full_raw(s), w.rb * BM + 32 * j, px, py, pn);
-#pragma unroll
-            for (int j = 0; j < GROUPS; ++j)
-              tma_4d(st + C::B_OFF + j * 4096, &mapG, full_raw(s), gch[j], p.stride_x * px + gdx[j],
-                     p.stride * py + gdy[j], pn);
-          }
-          __syncwarp();
-          if (++s == C::STAGES) { s = 0; ph ^= 1u; }
-        }
-      }
-      if (p.dbg && blockIdx.x == 0 && lane == 0) { p.dbg[0] = t_wait; p.dbg[1] = clock64() - t_all; }
-    }
-  } else if (warp == 1) {
-    // ===================== MMA issuer (whole warp converged, one elected lane issues: tc_common.cuh) ==========
-    if (rank == 0) {
-      // D fp32, A / B tf32, N = BN, M = 128 (256 over a CTA pair)
-      // (A lives in tensor memory: K-major by construction -- lane = row, column = K; B is MN-major, bit 16)
-      const unsigned idesc = (1u << 4) | (2u << 7) | (2u << 10) | (1u << 16) |
-                             ((unsigned)(BN >> 3) << 17) | ((unsigned)((CG * BM) >> 4) << 24);
-      int s = 0, acc = 0, sl = 0;
-      unsigned ph = 0, aph = 0;
-      long long t_wait_acc = 0, t_wait_ops = 0, t_all = clock64();
-      for (int item = first_item; item < total_items; item += item_step) {
-        const Item w = decode_item<CG>(p, item, rank);
-        const int iters = chunk_len(p, w.chunk);
-        for (int it = 0; it < iters; ++it) {
-          const int in_chunk = it % p.chunk;
-          if (in_chunk == 0) {
-            const long long t0 = clock64();
-            if (CG == 2) mbar_wait_cluster(tmem_empty(acc), aph ^ 1u); else mbar_wait(tmem_empty(acc), aph ^ 1u);
-            t_wait_acc += clock64() - t0;
-            tc_fence_after();
-          }
-          const unsigned d = tmem_base + (unsigned)(acc * BN);
-          const long long t1 = clock64();
-          if (CG == 2) {
-            mbar_wait_cluster(full_cvt(s), ph);      // the converter warps of both CTAs, each behind its own TMA barrier
-          } else {
-            mbar_wait(full_raw(s), ph);
-            mbar_wait(full_cvt(s), ph);
-          }
-          t_wait_ops += clock64() - t1;
-          tc_fence_after();
-          const unsigned st = base + s * C::STAGE_BYTES;
-          const unsigned long long b_hi = umma_desc_mn128(st + C::B_OFF, 4096);
-          const unsigned long long b_lo = umma_desc_mn128(st + C::B_OFF + C::B_BYTES, 4096);
-          const unsigned ta_hi = tmem_base + (unsigned)(C::ACC_COLS + sl * 2 * KP), ta_lo = ta_hi + KP;
-          if (elect_one()) {
-#pragma unroll
-          for (int k = 0; k < KP / 8; ++k) {            // A: 8 TMEM columns (pixels) per K step; B: 8 rows = 1024 B
-            const unsigned long long adv = (unsigned long long)(64 * k);
-            if (CG == 2) {
-              umma_tf32_ts_pair(d, ta_lo + 8 * k, b_hi + adv, idesc, (in_chunk | k) != 0);
-              umma_tf32_ts_pair(d, ta_hi + 8 * k, b_lo + adv, idesc, 1u);
-              umma_tf32_ts_pair(d, ta_hi + 8 * k, b_hi + adv, idesc, 1u);
-            } else {
-              umma_tf32_ts(d, ta_lo + 8 * k, b_hi + adv, idesc, (in_chunk | k) != 0);
-              umma_tf32_ts(d, ta_hi + 8 * k, b_lo + adv, idesc, 1u);
-              umma_tf32_ts(d, ta_hi + 8 * k, b_hi + adv, idesc, 1u);
-            }
-          }
-          if (CG == 2) umma_commit_pair(empty(s)); else umma_commit(empty(s));
-          if (CG == 2) umma_commit_pair(a_empty(sl)); else umma_commit(a_empty(sl));
-          if (in_chunk == p.chunk - 1 || it == iters - 1) {
-            if (CG == 2) umma_commit_pair(tmem_full(acc)); else umma_commit(tmem_full(acc));
-          }
-          }     // elect_one
-          __syncwarp();
-          if (++s == C::STAGES) { s = 0; ph ^= 1u; }
-          if (++sl == C::ASLOTS) sl = 0;
-          if (in_chunk == p.chunk - 1 || it == iters - 1) {
-            if (++acc == 2) { acc = 0; aph ^= 1u; }
-          }
-        }
-      }
-      if (p.dbg && blockIdx.x == 0 && lane == 0) { p.dbg[2] = t_wait_acc; p.dbg[3] = t_wait_ops; p.dbg[4] = clock64() - t_all; }
-    }
-  } else if (warp >= 4 && warp < 8) {
-    // ===================== P -> tensor memory =====================
-    // (Tried and removed: software-pipelining this role by one K block -- the next block's 32 values loaded before
-    // the current block's stores / G share / fences are waited for.  conv3_1: 747 instead of 555 us: the arrive of
-    // block i then waits for the TMA of block i + 1, and the MMA issuer starves.)
-    // warp = 32-channel group = TMEM lane quarter, lane = channel; column k of the operand = pixel k.
-    // (The G tile is split by all six converter warps, half here and half in warps 2-3: one warp per scheduler
-    // could not keep up with both tiles -- ncu: 45 % of the tensor pipe with the ALU pipe of the converter warps
-    // saturated -- and two warps alone cannot split 16 KB per K block in time either.)
-    int s = 0, sl = 0;
-    unsigned ph = 0, slph = 0;
-    long long t_wait = 0, t_wait_slot = 0, t_all = clock64();
-    for (int item = first_item; item < total_items; item += item_step) {
-      const Item w = decode_item<CG>(p, item, rank);
-      const int iters = chunk_len(p, w.chunk);
-      for (int it = 0; it < iters; ++it) {
-        { const long long t0 = clock64(); mbar_wait(full_raw(s), ph); t_wait += clock64() - t0; }
-        { const long long t0 = clock64(); mbar_wait(a_empty(sl), slph ^ 1u); t_wait_slot += clock64() - t0; }   // MMAs done with this slot
-        tc_fence_after();
-        const float *grp = reinterpret_cast<const float *>(gbase + s * C::STAGE_BYTES + (warp & 3) * 4096) + lane;
-        unsigned hi[KP], lo[KP];
-#pragma unroll
-        for (int k = 0; k < KP; ++k) {
-          const float v = grp[k * 32];
-          if (p.trunc) {
-            hi[k] = __float_as_uint(v);
-            lo[k] = __float_as_uint(v - __uint_as_float(__float_as_uint(v) & 0xFFFFE000u));
-          } else {
-            const float h = tf32_rna_fast(v);
-            hi[k] = __float_as_uint(h);
-            lo[k] = __float_as_uint(v - h);
-          }
-        }
-        const unsigned ta = tmem_base + ((unsigned)((warp & 3) * 32) << 16) + (unsigned)(C::ACC_COLS + sl * 2 * KP);
-        tmem_st32(ta, hi);
-        tmem_st32(ta + KP, lo);
-        {                                    // ... and the first half of G (warps 2-3 take the second half)
-          float4 *a = reinterpret_cast<float4 *>(gbase + s * C::STAGE_BYTES + C::B_OFF);
-          float4 *l = reinterpret_cast<float4 *>(gbase + s * C::STAGE_BYTES + C::B_OFF + C::B_BYTES);
-#pragma unroll
-          for (int i = threadIdx.x - 128; i < p.g_first; i += 128) {
-            const float4 v = a[i];
-            float4 h, r;
-            if (p.trunc) {
-              r.x = v.x - __uint_as_float(__float_as_uint(v.x) & 0xFFFFE000u); r.y = v.y - __uint_as_float(__float_as_uint(v.y) & 0xFFFFE000u);
-              r.z = v.z - __uint_as_float(__float_as_uint(v.z) & 0xFFFFE000u); r.w = v.w - __uint_as_float(__float_as_uint(v.w) & 0xFFFFE000u);
-              l[i] = r;
-              continue;
-            }
-            h.x = tf32_rna_fast(v.x); h.y = tf32_rna_fast(v.y); h.z = tf32_rna_fast(v.z); h.w = tf32_rna_fast(v.w);
-            r.x = v.x - h.x; r.y = v.y - h.y; r.z = v.z - h.z; r.w = v.w - h.w;
-            a[i] = h;
-            l[i] = r;
-          }
-          fence_proxy_async();
-        }
-        asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) {
-          if (CG == 2) mbar_arrive_cta(full_cvt(s), 0); else mbar_arrive(full_cvt(s));
-        }
-        if (++s == C::STAGES) { s = 0; ph ^= 1u; }
-        if (++sl == C::ASLOTS) { sl = 0; slph ^= 1u; }
-      }
-    }
-    if (p.dbg && blockIdx.x == 0 && threadIdx.x == 128) { p.dbg[5] = t_wait; p.dbg[6] = clock64() - t_all; p.dbg[9] = t_wait_slot; }
-  } else if (warp == 2 || warp == 3 || warp >= 16) {
-    // ===================== G split in shared memory: hi in place, lo beside it =====================
-    const int tid = (warp < 4 ? warp - 2 : warp - 14) * 32 + lane;     // 0..191
     int s = 0;
     unsigned ph = 0;
-    for (int item = first_item; item < total_items; item += item_step) {
-      const Item w = decode_item<CG>(p, item, rank);
-      const int iters = chunk_len(p, w.chunk);
-      for (int it = 0; it < iters; ++it) {
-        mbar_wait(full_raw(s), ph);
-        unsigned char *stp = gbase + s * C::STAGE_BYTES;
-        float4 *a = reinterpret_cast<float4 *>(stp + C::B_OFF);
-        float4 *l = reinterpret_cast<float4 *>(stp + C::B_OFF + C::B_BYTES);
+    long long t_wait = 0, t_all = clock64();
+    for (int item = blockIdx.x; item < total_items; item += gridDim.x) {
+      const Item w = decode_item(p, item);
+      int gch[GROUPS], gdx[GROUPS], gdy[GROUPS];           // per column group: channel, tap offset
 #pragma unroll
-        for (int i = p.g_first + tid; i < C::B_BYTES / 16; i += 32 * GWARPS) {
-          const float4 v = a[i];
-          float4 h, r;
-          if (p.trunc) {
-            r.x = v.x - __uint_as_float(__float_as_uint(v.x) & 0xFFFFE000u); r.y = v.y - __uint_as_float(__float_as_uint(v.y) & 0xFFFFE000u);
-            r.z = v.z - __uint_as_float(__float_as_uint(v.z) & 0xFFFFE000u); r.w = v.w - __uint_as_float(__float_as_uint(v.w) & 0xFFFFE000u);
-            l[i] = r;
-            continue;
-          }
-          h.x = tf32_rna_fast(v.x); h.y = tf32_rna_fast(v.y); h.z = tf32_rna_fast(v.z); h.w = tf32_rna_fast(v.w);
-          r.x = v.x - h.x; r.y = v.y - h.y; r.z = v.z - h.z; r.w = v.w - h.w;
-          a[i] = h;
-          l[i] = r;
+      for (int j = 0; j < GROUPS; ++j) {
+        const int v = w.cb * GROUPS + j;
+        if (v < p.vgroups) {
+          const int tap = v / p.cgroups, ky = tap / p.kw;
+          gch[j] = (v - tap * p.cgroups) * 32; gdy[j] = ky - p.pad_t; gdx[j] = tap - ky * p.kw - p.pad_l;
+        } else {
+          gch[j] = p.cgroups * 32; gdx[j] = gdy[j] = 0;    // past the last group: channels >= C, TMA zero fill
         }
-        fence_proxy_async();
+      }
+      const int k0 = w.chunk * p.kc, klen = chunk_len(p, w.chunk);
+      for (int kb = k0; kb < k0 + klen; ++kb) {
+        int q = kb;
+        const int px = (q % p.tiles_x) * p.TW; q /= p.tiles_x;
+        const int py = (q % p.tiles_y) * p.TH; q /= p.tiles_y;
+        const int pn = q * p.TN;
+        { const long long t0 = clock64(); mbar_wait(empty(s), ph ^ 1u); t_wait += clock64() - t0; }
+        const unsigned st = base + s * C::STAGE_BYTES;
+        if (elect_one()) {
+          mbar_expect_tx(full(s), (unsigned)(A_BYTES + C::G_BYTES));
+#pragma unroll
+          for (int j = 0; j < BM / 32; ++j)       // channels past R are TMA zero fill
+            tma_4d(st + j * 4096, &mapP, full(s), w.rb * BM + 32 * j, px, py, pn);
+#pragma unroll
+          for (int j = 0; j < GROUPS; ++j)
+            tma_4d(st + C::G_RAW + j * 4096, &mapG, full(s), gch[j], p.stride_x * px + gdx[j],
+                   p.stride * py + gdy[j], pn);
+        }
         __syncwarp();
-        if (lane == 0) {
-          if (CG == 2) mbar_arrive_cta(full_cvt(s), 0); else mbar_arrive(full_cvt(s));
-        }
         if (++s == C::STAGES) { s = 0; ph ^= 1u; }
       }
     }
-  } else if (warp >= 8 && warp < 16) {
-    // ===================== epilogue: fp32 register accumulation, then red.add into dW =====================
-    constexpr int COLS = BN / 2;
-    const int q = warp & 3;
-    const int half = (warp - 8) >> 2;
-    const int row = q * 32 + lane;
-    int acc = 0;
-    unsigned aph = 0;
+    if (p.dbg && blockIdx.x == 0 && lane == 0) { p.dbg[0] = t_wait; p.dbg[1] = clock64() - t_all; }
+  } else if (warp >= 4) {
+    // ===================== consumers: split + transpose, wgmma, red.add into dW =====================
+    const int cw = (warp >> 2) - 1;                  // rows [64 cw, 64 cw + 64) of the 128-row block
+    const int ct = threadIdx.x - 128 * (cw + 1);
+    const int row0 = 64 * cw + 16 * (ct >> 5) + (lane >> 2);
+    const int col0 = 2 * (lane & 3);
+    int s = 0;
+    unsigned ph = 0;
     long long t_wait = 0, t_all = clock64();
-    for (int item = first_item; item < total_items; item += item_step) {
-      const Item w = decode_item<CG>(p, item, rank);
+    float sum[R], acc[R];
+    for (int item = blockIdx.x; item < total_items; item += gridDim.x) {
+      const Item w = decode_item(p, item);
       const int iters = chunk_len(p, w.chunk);
-      const int chunks = (iters + p.chunk - 1) / p.chunk;
-      float sum[COLS];
 #pragma unroll
-      for (int c = 0; c < COLS; ++c) sum[c] = 0.f;
-      for (int ck = 0; ck < chunks; ++ck) {
-        { const long long t0 = clock64(); mbar_wait(tmem_full(acc), aph); t_wait += clock64() - t0; }
-        tc_fence_after();
-        const unsigned taddr = tmem_base + ((unsigned)(q * 32) << 16) + (unsigned)(acc * BN + half * COLS);
+      for (int c = 0; c < R; ++c) sum[c] = 0.f;
+      int pending = -1;
+      for (int it = 0; it < iters; ++it) {
+        const int in_chunk = it % p.chunk;
+        const bool chunk_end = in_chunk == p.chunk - 1 || it == iters - 1;
+        { const long long t0 = clock64(); mbar_wait(full(s), ph); t_wait += clock64() - t0; }
+        unsigned char *stp = gbase + s * C::STAGE_BYTES;
+        split_transpose<64>(reinterpret_cast<const float *>(stp), stp + C::A_HI, stp + C::A_LO, 64 * cw, ct);
+        split_transpose<BN / 2>(reinterpret_cast<const float *>(stp + C::G_RAW), stp + C::B_HI, stp + C::B_LO,
+                                cw * (BN / 2), ct);
+        fence_proxy_async();
+        named_bar_sync(1, 256);                      // both halves of G are split
+        const unsigned st = base + s * C::STAGE_BYTES;
+        const unsigned long long a_hi = wgmma_desc_k128(st + C::A_HI + cw * (A_BYTES / 2));
+        const unsigned long long a_lo = wgmma_desc_k128(st + C::A_LO + cw * (A_BYTES / 2));
+        const unsigned long long b_hi = wgmma_desc_k128(st + C::B_HI), b_lo = wgmma_desc_k128(st + C::B_LO);
+        fence_regs(acc);
+        wgmma_fence();
 #pragma unroll
-        for (int c0 = 0; c0 < COLS; c0 += 16) {
-          unsigned r[16];
-          tmem_ld16(taddr + (unsigned)c0, r);
-#pragma unroll
-          for (int e = 0; e < 16; ++e) sum[c0 + e] += __uint_as_float(r[e]);
+        for (int k = 0; k < KP / 8; ++k) {
+          const unsigned long long adv = (unsigned long long)(2 * k);
+          Wgmma<BN>::mma(acc, a_lo + adv, b_hi + adv, (in_chunk | k) != 0);
+          Wgmma<BN>::mma(acc, a_hi + adv, b_lo + adv, 1);
+          Wgmma<BN>::mma(acc, a_hi + adv, b_hi + adv, 1);
         }
-        tc_fence_before();
+        wgmma_commit();
+        if (chunk_end) wgmma_wait<0>(); else wgmma_wait<1>();
+        fence_regs(acc);
         __syncwarp();
-        if (lane == 0) {
-          if (CG == 2) mbar_arrive_cta(tmem_empty(acc), 0); else mbar_arrive(tmem_empty(acc));
+        if (pending >= 0 && lane == 0) mbar_arrive(empty(pending));
+        pending = s;
+        if (chunk_end) {
+          if (lane == 0) mbar_arrive(empty(s));
+          pending = -1;
+#pragma unroll
+          for (int c = 0; c < R; ++c) sum[c] += acc[c];
         }
-        if (++acc == 2) { acc = 0; aph ^= 1u; }
+        if (++s == C::STAGES) { s = 0; ph ^= 1u; }
       }
-      const int r = w.rb * BM + row;
-      if (r < p.R) {
 #pragma unroll
-        for (int g = 0; g < (COLS + 31) / 32; ++g) {       // the (tap, channel group) pairs this thread holds
-          const int col0 = half * COLS + 32 * g;             // column within the BN block
-          const int v = w.cb * (BN / 32) + col0 / 32;
-          if (v < p.vgroups) {
-            const int tap = v / p.cgroups, c0 = (v - tap * p.cgroups) * 32 + (col0 & 31);
-            float *dst = p.dw + (long long)r * p.pitch_r + (long long)tap * p.pitch_t + c0;
+      for (int h = 0; h < 2; ++h) {
+        const int r = w.rb * BM + row0 + 8 * h;
+        if (r >= p.R) continue;
 #pragma unroll
-            for (int c = 0; c < (COLS < 32 ? COLS : 32); ++c)
-              if (c0 + c < p.C) red_add_f32(dst + c, sum[32 * g + c]);
-          }
+        for (int j = 0; j < BN / 8; ++j) {
+          const int col = 8 * j + col0;              // column within the BN block; col, col + 1 share a group
+          const int v = w.cb * GROUPS + col / 32;
+          if (v >= p.vgroups) continue;
+          const int tap = v / p.cgroups, c = (v - tap * p.cgroups) * 32 + (col & 31);
+          float *dst = p.dw + (long long)r * p.pitch_r + (long long)tap * p.pitch_t + c;
+          if (c < p.C) red_add_f32(dst, sum[4 * j + 2 * h]);
+          if (c + 1 < p.C) red_add_f32(dst + 1, sum[4 * j + 2 * h + 1]);
         }
       }
     }
-    if (p.dbg && blockIdx.x == 0 && threadIdx.x == 256) { p.dbg[7] = t_wait; p.dbg[8] = clock64() - t_all; }
-  }
-  tc_fence_before();
-  if (CG == 2) cluster_sync_all(); else __syncthreads();
-  if (warp == 2) {
-    if (CG == 2)
-      asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((unsigned)C::TMEM_COLS) : "memory");
-    else
-      asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((unsigned)C::TMEM_COLS) : "memory");
+    if (p.dbg && blockIdx.x == 0 && threadIdx.x == 128) { p.dbg[2] = t_wait; p.dbg[3] = clock64() - t_all; }
   }
 }
 
-int g_wgrad_trunc = 0;    // unflow_set_int_option("tc_wgrad_trunc"): experiment, see WgradParams::trunc
-int g_wgrad_gsplit = 2;   // unflow_set_int_option("tc_wgrad_gsplit"): share of the G tile split by warps 4-7: 0 = none, 3 = a quarter, 1 / 2 = half (default)
-
-template <int BN, int CG>
-static int launch_v(const CUtensorMap &mP, const CUtensorMap &mG, const WgradParams &p, cudaStream_t stream) {
-  using C = Cfg<BN, CG>;
+template <int BN>
+static int launch(const CUtensorMap &mP, const CUtensorMap &mG, const WgradParams &p, cudaStream_t stream) {
+  using C = Cfg<BN>;
   static bool attr_set = false;
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(tc_wgrad_kernel<BN, CG>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES);
+    cudaError_t e = cudaFuncSetAttribute(tc_wgrad_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES);
     if (e != cudaSuccess) { set_error("tc_wgrad: cannot opt in to %d bytes of shared memory: %s", C::SMEM_BYTES, cudaGetErrorString(e)); return UNFLOW_ECUDA; }
     attr_set = true;
   }
-  const long long total = (long long)p.n_chunks * (CG == 2 ? (p.r_blocks + 1) / 2 : p.r_blocks) * p.c_blocks;
-  // Who splits the G tile?  The role timers (tools/tc_conv_check.py --roles) show the P-converter warps 4-7 busy
-  // 85 % and the MMA issuer waiting 40 % for operands in the pair kernel, so the converter warps are what bounds
-  // it; but the two spare warps cannot take more of the G tile than half (conv3_1, pairs: half 580 us, three
-  // quarters 610 us, all of it 670 us): half / half stays.
-  WgradParams q = p;
-  q.trunc = g_wgrad_trunc;
-  q.g_first = (g_wgrad_gsplit == 0 || g_wgrad_gsplit == 2) ? 0 : g_wgrad_gsplit == 3 ? C::B_BYTES / 64 : C::B_BYTES / 32;
-  if (CG == 2) {
-    const int pairs = total < kNumSMs / 2 ? (int)total : kNumSMs / 2;
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(2 * pairs); cfg.blockDim = dim3(NTHREADS); cfg.dynamicSmemBytes = C::SMEM_BYTES; cfg.stream = stream;
-    cudaLaunchAttribute at[1];
-    at[0].id = cudaLaunchAttributeClusterDimension;
-    at[0].val.clusterDim.x = 2; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
-    cfg.attrs = at; cfg.numAttrs = 1;
-    cudaError_t e = cudaLaunchKernelEx(&cfg, tc_wgrad_kernel<BN, CG>, mP, mG, q);
-    if (e != cudaSuccess) { set_error("tc_wgrad: cluster launch failed: %s", cudaGetErrorString(e)); return UNFLOW_ECUDA; }
-  } else {
-    const int grid = total < kNumSMs ? (int)total : kNumSMs;
-    tc_wgrad_kernel<BN, CG><<<grid, NTHREADS, C::SMEM_BYTES, stream>>>(mP, mG, q);
-  }
+  const long long total = (long long)p.n_chunks * p.r_blocks * p.c_blocks;
+  const int grid = total < kNumSMs ? (int)total : kNumSMs;
+  tc_wgrad_kernel<BN><<<grid, NTHREADS, C::SMEM_BYTES, stream>>>(mP, mG, p);
   count_launch();
   return check_launch("tc_wgrad_kernel");
 }
 
-// CTA pairs (see Cfg) whenever there are at least two row blocks to pair and the full-width tile
-// (unflow_set_int_option("tc_pair", 0) switches them off)
 static int launch_bn(int BN, const CUtensorMap &mP, const CUtensorMap &mG, const WgradParams &p, cudaStream_t stream) {
-  if (BN == 128 && p.r_blocks >= 2 && g_pair != 0) return launch_v<128, 2>(mP, mG, p, stream);
-  if (BN == 128) return launch_v<128, 1>(mP, mG, p, stream);
-  if (BN == 64) return launch_v<64, 1>(mP, mG, p, stream);
-  return launch_v<32, 1>(mP, mG, p, stream);
+  if (BN == 128) return launch<128>(mP, mG, p, stream);
+  if (BN == 64) return launch<64>(mP, mG, p, stream);
+  return launch<32>(mP, mG, p, stream);
 }
 
 // the K-block pixel box: TW*TH*TN == 32 exactly (rows past the tensor are TMA zero fill), fewest boxes
@@ -527,8 +304,6 @@ static int make_plan(WgradParams &p, int &BN, int N, int Hp, int Wp, int R, int 
 }
 
 }  // namespace tcw
-int set_tc_wgrad_trunc(int v) { if (v != 0 && v != 1) return 0; tcw::g_wgrad_trunc = v; return 1; }
-int set_tc_wgrad_gsplit(int v) { if (v < 0 || v > 3) return 0; tcw::g_wgrad_gsplit = v; return 1; }
 }  // namespace unflow
 
 using namespace unflow;
@@ -565,7 +340,7 @@ extern "C" int unflow_tc_wgrad(const float *P, int N, int Hp, int Wp, int R, lon
     cuuint64_t strides[3] = {(cuuint64_t)p_pitch * 4, (cuuint64_t)p_pitch * 4 * Wp, (cuuint64_t)p_pitch * 4 * Wp * Hp};
     cuuint32_t box[4] = {32, (cuuint32_t)p.TW, (cuuint32_t)p.TH, (cuuint32_t)p.TN};
     cuuint32_t estr[4] = {1, 1, 1, 1};
-    rc = tc::encode(&mP, P, 4, dims, strides, box, estr, CU_TENSOR_MAP_SWIZZLE_NONE);   // read by the converter warps only
+    rc = tc::encode(&mP, P, 4, dims, strides, box, estr, CU_TENSOR_MAP_SWIZZLE_NONE);   // split + transposed by the consumers
     if (rc) return rc;
   }
   {
@@ -573,7 +348,7 @@ extern "C" int unflow_tc_wgrad(const float *P, int N, int Hp, int Wp, int R, lon
     cuuint64_t strides[3] = {(cuuint64_t)g_pitch * 4, (cuuint64_t)g_pitch * 4 * Wg, (cuuint64_t)g_pitch * 4 * Wg * Hg};
     cuuint32_t box[4] = {32, (cuuint32_t)(p.TW * stride), (cuuint32_t)(p.TH * stride), (cuuint32_t)p.TN};
     cuuint32_t estr[4] = {1, (cuuint32_t)stride, (cuuint32_t)stride, 1};
-    rc = tc::encode(&mG, G, 4, dims, strides, box, estr, CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B);
+    rc = tc::encode(&mG, G, 4, dims, strides, box, estr, CU_TENSOR_MAP_SWIZZLE_NONE);
     if (rc) return rc;
   }
   return tcw::launch_bn(BN, mP, mG, p, (cudaStream_t)stream);
@@ -602,7 +377,7 @@ extern "C" int unflow_tc_wgrad_window(const float *P, int N, int Ho, int Wo, int
     cuuint64_t strides[3] = {(cuuint64_t)p_pitch * 4, (cuuint64_t)p_pitch * 4 * Wo, (cuuint64_t)p_pitch * 4 * Wo * Ho};
     cuuint32_t box[4] = {32, (cuuint32_t)p.TW, (cuuint32_t)p.TH, (cuuint32_t)p.TN};
     cuuint32_t estr[4] = {1, 1, 1, 1};
-    rc = tc::encode(&mP, P, 4, dims, strides, box, estr, CU_TENSOR_MAP_SWIZZLE_NONE);   // read by the converter warps only
+    rc = tc::encode(&mP, P, 4, dims, strides, box, estr, CU_TENSOR_MAP_SWIZZLE_NONE);   // split + transposed by the consumers
     if (rc) return rc;
   }
   {
@@ -610,7 +385,7 @@ extern "C" int unflow_tc_wgrad_window(const float *P, int N, int Ho, int Wo, int
     cuuint64_t strides[3] = {(cuuint64_t)stride * Cp * 4, (cuuint64_t)Wp * Cp * 4, (cuuint64_t)Wp * Cp * 4 * H};
     cuuint32_t box[4] = {32, (cuuint32_t)p.TW, (cuuint32_t)(p.TH * stride), (cuuint32_t)p.TN};
     cuuint32_t estr[4] = {1, 1, (cuuint32_t)stride, 1};
-    rc = tc::encode(&mG, xp, 4, dims, strides, box, estr, CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B);
+    rc = tc::encode(&mG, xp, 4, dims, strides, box, estr, CU_TENSOR_MAP_SWIZZLE_NONE);
     if (rc) return rc;
   }
   return tcw::launch_bn(BN, mP, mG, p, (cudaStream_t)stream);

@@ -4,7 +4,7 @@
           no tensor cores.
 '3xtf32'  the same contraction on the tensor cores at fp32-level accuracy (the default of bench.py and the
           trainer): every operand is split x = hi + lo (hi = TF32-rounded, lo = exact residual) and
-          lo*hi' + hi*lo' + hi*hi' is accumulated by the hand-written tcgen05 kernels (csrc/tc_conv.cu: forward
+          lo*hi' + hi*lo' + hi*hi' is accumulated by the hand-written wgmma kernels (csrc/tc_conv.cu: forward
           and input gradient, csrc/tc_wgrad.cu: weight gradient, csrc/narrow_conv*.cu: the 2-channel flow
           heads in exact fp32) with the K loop cut into chunks that are summed in fp32 registers: 1.8e-6 of
           max|y| against float64 per layer, and the same 1e-4 flow tolerance against the fp32 oracle as the
@@ -167,7 +167,7 @@ def _conv_input_grad(input_hw, weight, grad_output, stride):
     strided conv leaves unused).  ``torch.nn.grad.conv2d_input`` computes the same thing but hands
     cuDNN a stride-0 placeholder for ``x``; ATen then aligns ``grad_output`` to THAT tensor's
     (NCHW) format and back to the weight's NHWC -- two full copies of the 3x-wide gradient operand
-    per layer, 2.4 ms of the 26 ms step in the ncu launch list (profiles/)."""
+    per layer."""
     sh, sw = (stride, stride) if isinstance(stride, int) else stride
     kh, kw = weight.shape[2], weight.shape[3]
     oph = input_hw[0] - ((grad_output.shape[2] - 1) * sh + kh)
@@ -292,7 +292,7 @@ class _Deconv3x(torch.autograd.Function):
 
 
 # ---------------------------------------------------------------------------------------------
-# Hand-written tensor-core path (csrc/tc_conv.cu): tcgen05 implicit GEMM, 3xTF32 split in shared
+# Hand-written tensor-core path (csrc/tc_conv.cu): wgmma implicit GEMM, 3xTF32 split in shared
 # memory, fused bias / leaky ReLU.  Forward and input gradient; the weight gradient still goes
 # through the library path below (round-2 work in progress: csrc/tc_wgrad).
 # ---------------------------------------------------------------------------------------------
@@ -406,7 +406,7 @@ def _input_grad_into_slot(gen, x, launch):
 
 
 class _ConvTC(torch.autograd.Function):
-    """slim.conv2d on the hand-written tcgen05 kernel: y = act(conv(x, w; stride, TF SAME) + b)."""
+    """slim.conv2d on the hand-written wgmma kernel: y = act(conv(x, w; stride, TF SAME) + b)."""
 
     @staticmethod
     def forward(ctx, x, w, b, stride, pads, act, out=None):
@@ -419,7 +419,6 @@ class _ConvTC(torch.autograd.Function):
         planes = tc_conv.split_weights(_khwc(w))
         tc_conv.run(x, planes, dst, mode=0, stride=stride, kh=k, kw=k, pad_t=pt, pad_l=pl,
                     bias=b, act=bool(act))
-        ctx.planes = planes if _REUSE_PLANES else None      # the input gradient reads the same planes (MN-major)
         ctx.save_for_backward(x, w, y if act else None)
         ctx.cfg = (stride, tuple(pads), b is not None, bool(act))
         ctx.gen = _generation
@@ -439,10 +438,9 @@ class _ConvTC(torch.autograd.Function):
             gb = gb_all
         if ctx.needs_input_grad[0]:
             # dx = conv_transpose(gpre, w): rows of the GEMM = C_in, contraction = C_out
-            planes, ctx.planes = getattr(ctx, 'planes', None), None
             gx = _input_grad_into_slot(ctx.gen, x, lambda dst, acc: tc_conv.run(
-                gpre, planes if planes is not None else tc_conv.split_weights(_khwc(w), transpose=True), dst, mode=1,
-                stride=stride, kh=k, kw=k, pad_t=pt, pad_l=pl, accumulate=acc, planes_t=planes is not None))
+                gpre, tc_conv.split_weights(_khwc(w), transpose=True), dst, mode=1,
+                stride=stride, kh=k, kw=k, pad_t=pt, pad_l=pl, accumulate=acc))
         if ctx.needs_input_grad[1]:
             if _TC_WGRAD and tc_conv.supported(gpre):
                 gw = _tc_weight_grad(gpre, x, w, stride, pt, pl)                   # rows C_out, columns C_in
@@ -495,9 +493,6 @@ class _ConvWindow(torch.autograd.Function):
 
 
 _WINDOW = __import__('os').environ.get('UNFLOW_CONV1_WINDOW', '1') != '0'
-# the input-gradient launch of a layer reads the hi / lo weight planes its forward launch split (as MN-major B
-# tiles) instead of splitting a transposed pair: half the wsplit launches of a step (UNFLOW_REUSE_PLANES=0: off)
-_REUSE_PLANES = __import__('os').environ.get('UNFLOW_REUSE_PLANES', '1') != '0'
 
 
 def _use_window(x, w, stride):
@@ -517,7 +512,6 @@ class _DeconvTC(torch.autograd.Function):
         dst, y = _dest(out, N, Co, 2 * H, 2 * W, x.device)
         planes = tc_conv.split_weights(_khwc(w), transpose=True)
         tc_conv.run(x, planes, dst, mode=1, stride=2, kh=4, kw=4, pad_t=1, pad_l=1, bias=b, act=bool(act))
-        ctx.planes = planes if _REUSE_PLANES else None
         ctx.save_for_backward(x, w, y if act else None)
         ctx.cfg = (b is not None, bool(act))
         ctx.gen = _generation
@@ -536,10 +530,9 @@ class _DeconvTC(torch.autograd.Function):
             gb = gb_all
         if ctx.needs_input_grad[0]:
             # dx = conv(gpre, w; stride 2, pad 1): rows = C_in (dim 0 of the IOHW variable), contraction = C_out
-            planes, ctx.planes = getattr(ctx, 'planes', None), None
             gx = _input_grad_into_slot(ctx.gen, x, lambda dst, acc: tc_conv.run(
-                gpre, planes if planes is not None else tc_conv.split_weights(_khwc(w)), dst, mode=0, stride=2, kh=4,
-                kw=4, pad_t=1, pad_l=1, accumulate=acc, planes_t=planes is not None))
+                gpre, tc_conv.split_weights(_khwc(w)), dst, mode=0, stride=2, kh=4,
+                kw=4, pad_t=1, pad_l=1, accumulate=acc))
         if ctx.needs_input_grad[1]:
             if _TC_WGRAD and tc_conv.supported(gpre):
                 gw = _tc_weight_grad(x, gpre, w, 2, 1, 1)                          # rows C_in, columns C_out

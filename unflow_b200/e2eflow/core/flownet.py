@@ -12,7 +12,7 @@ Differences in mechanism, not in results:
     passes over B -- same arithmetic per sample, half the launches, larger GEMMs.
   * conv / deconv stacks run on cuDNN through torch (dense contractions; fp32 accumulate),
     with TF ``SAME`` padding reproduced exactly (asymmetric for the stride-2 layers).
-  * ``correlation`` and ``image_warp`` are the hand-written sm_100a kernels.
+  * ``correlation`` and ``image_warp`` are the hand-written sm_90a kernels.
 """
 import math
 

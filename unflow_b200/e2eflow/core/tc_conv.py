@@ -1,4 +1,4 @@
-"""Host side of csrc/tc_conv.cu: the hand-written tcgen05 (3xTF32, TMEM accumulators) implicit-GEMM
+"""Host side of csrc/tc_conv.cu: the hand-written wgmma (3xTF32, register accumulators) implicit-GEMM
 convolution behind the conv / deconv stacks (reference slim.conv2d / slim.conv2d_transpose,
 src/e2eflow/core/flownet.py:166-233, :89-155).
 
@@ -75,7 +75,7 @@ def split_weights(w, transpose=False):
 
 
 def run(x, planes, out, *, mode, stride, kh, kw, pad_t, pad_l, bias=None, act=False, accumulate=False,
-        slope=0.1, planes_t=False):
+        slope=0.1):
     """out (+)= act(bias + conv(x)) -- ``x`` / ``out``: NCHW-shaped tensors with NHWC memory (channel
     slices allowed).  mode 0: convolution with offsets (pad_t, pad_l); mode 1: transposed convolution
     (o = stride * i - pad + k)."""
@@ -83,12 +83,7 @@ def run(x, planes, out, *, mode, stride, kh, kw, pad_t, pad_l, bias=None, act=Fa
     assert gx is not None and go is not None, "tc_conv needs NHWC (channels_last) memory"
     N, Hin, Win, Cin, xp = gx
     No, Hout, Wout, Cout, yp = go
-    # planes_t: ``planes`` were split for the layer's other direction (rows = this call's contraction): the
-    # input gradient reuses the forward pass's planes instead of splitting a transposed pair
-    if planes_t:
-        assert No == N and planes.rows == Cin and planes.cols == Cout and planes.taps == kh * kw
-    else:
-        assert No == N and planes.rows == Cout and planes.cols == Cin and planes.taps == kh * kw
+    assert No == N and planes.rows == Cout and planes.cols == Cin and planes.taps == kh * kw
     from ..ops import kernel_timer
     pix = N * (Hin * Win if mode == 1 else Hout * Wout)       # positions each tap is applied to
     flops = 2 * pix * Cout * Cin * kh * kw            # nominal fp32 multiply-adds x 2 (executed as 3 TF32 MMAs each)
@@ -96,7 +91,7 @@ def run(x, planes, out, *, mode, stride, kh, kw, pad_t, pad_l, bias=None, act=Fa
         check(_native.lib().unflow_tc_conv(
             x.data_ptr(), N, Hin, Win, Cin, xp, planes.hi.data_ptr(), planes.lo.data_ptr(),
             out.data_ptr(), Hout, Wout, Cout, yp, bias.data_ptr() if bias is not None else None,
-            float(slope), 1 if act else 0, 1 if accumulate else 0, mode | (2 if planes_t else 0), stride, kh, kw,
+            float(slope), 1 if act else 0, 1 if accumulate else 0, mode, stride, kh, kw,
             pad_t, pad_l, _stream()), "tc_conv")
     return out
 

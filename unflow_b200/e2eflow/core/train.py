@@ -71,9 +71,8 @@ class Trainer:
         train.py:160,169).  run.py trains with it on; bench.py and the parity tests keep it off
         (random draws cannot be parity-pinned).  The draws come from the device generator so the
         step stays capturable in a CUDA graph."""
-        # bucketed all-reduce on a side stream behind the backward checkpoints: OFF by default -- measured on
-        # 2 and 8 B200s it is 0.07 / 0.22 ms per step SLOWER than one all-reduce after the backward pass (the
-        # persistent conv kernels hold all 148 SMs, NCCL's kernels wait for them either way; profiles/r2_bench.md)
+        # bucketed all-reduce on a side stream behind the backward checkpoints: OFF by default -- the persistent
+        # conv kernels hold every SM, so NCCL's kernels wait for them either way
         self.overlap_allreduce = __import__('os').environ.get('UNFLOW_OVERLAP_ALLREDUCE', '0') != '0'
         self.augment = bool(augment)
         if self.augment:
