@@ -141,7 +141,9 @@ tc_conv_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
   auto full = [&](int s) { return bars + 8u * s; };                   // stage s landed (TMA)
   auto empty = [&](int s) { return bars + 8u * (C::STAGES + s); };    // stage s consumed (MMAs of both consumers done)
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  // warp index made warp-uniform for ptxas: with a plain threadIdx.x >> 5 it cannot prove the role branch is uniform
+  // across a warpgroup, treats the wgmma code as divergent and waits for every MMA before issuing the next (C7518)
+  const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0), lane = threadIdx.x & 31;
   const int m_tiles = p.tiles_n * p.tiles_y * p.tiles_x;
   const int total_items = p.n_classes * m_tiles * p.n_blocks * p.ksplit;
 
@@ -209,52 +211,58 @@ tc_conv_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
       const int iters = wk.iters;
 #pragma unroll
       for (int c = 0; c < R; ++c) sum[c] = 0.f;
-      int pending = -1;                              // stage whose MMAs may still be running
-      for (int it = 0; it < iters; ++it) {
-        const int in_chunk = it % p.chunk;
-        const bool chunk_end = in_chunk == p.chunk - 1 || it == iters - 1;
-        { const long long t0 = clock64(); mbar_wait(full(s), ph); t_wait += clock64() - t0; }
-        // split this warpgroup's 64 rows (8 KB): the elementwise split keeps the swizzled positions
-        {
-          float4 *a = reinterpret_cast<float4 *>(gbase + s * C::STAGE_BYTES + cw * (A_BYTES / 2));
-          float4 *l = reinterpret_cast<float4 *>(gbase + s * C::STAGE_BYTES + A_BYTES + cw * (A_BYTES / 2));
+      // Outer loop over chunks, inner loop over the K blocks of a chunk.  The inner loop only ever waits for the
+      // previous K block's MMAs (wait_group 1), so they overlap this block's split; the accumulator is read only
+      // after the inner loop, behind wait_group 0.  A read of acc inside the inner loop would make ptxas wait for
+      // every MMA group (C7517).
+      for (int c0 = 0; c0 < iters; c0 += p.chunk) {
+        const int c1 = c0 + p.chunk < iters ? c0 + p.chunk : iters;
+        int pending = -1;                            // stage whose MMAs may still be running
+        for (int it = c0; it < c1; ++it) {
+          { const long long t0 = clock64(); mbar_wait(full(s), ph); t_wait += clock64() - t0; }
+          // split this warpgroup's 64 rows (8 KB): the elementwise split keeps the swizzled positions
+          {
+            float4 *a = reinterpret_cast<float4 *>(gbase + s * C::STAGE_BYTES + cw * (A_BYTES / 2));
+            float4 *l = reinterpret_cast<float4 *>(gbase + s * C::STAGE_BYTES + A_BYTES + cw * (A_BYTES / 2));
 #pragma unroll
-          for (int j = 0; j < A_BYTES / 2 / 16 / 128; ++j) {
-            const int i = ct + 128 * j;
-            const float4 v = a[i], h = tf32_hi4(v);
-            a[i] = h;
-            l[i] = sub4(v, h);
+            for (int j = 0; j < A_BYTES / 2 / 16 / 128; ++j) {
+              const int i = ct + 128 * j;
+              const float4 v = a[i], h = tf32_hi4(v);
+              a[i] = h;
+              l[i] = sub4(v, h);
+            }
           }
-        }
-        fence_proxy_async();                         // generic-proxy writes -> visible to the tensor core
-        named_bar_sync(1 + cw, 128);
-        const unsigned st = base + s * C::STAGE_BYTES;
-        const unsigned long long a_hi = wgmma_desc_k128(st + cw * (A_BYTES / 2));
-        const unsigned long long a_lo = wgmma_desc_k128(st + A_BYTES + cw * (A_BYTES / 2));
-        const unsigned long long b_hi = wgmma_desc_k128(st + C::B_OFF), b_lo = wgmma_desc_k128(st + C::B_OFF + C::B_BYTES);
-        fence_regs(acc);
-        wgmma_fence();
+          fence_proxy_async();                       // generic-proxy writes -> visible to the tensor core
+          named_bar_sync(1 + cw, 128);
+          const unsigned st = base + s * C::STAGE_BYTES;
+          const unsigned long long a_hi = wgmma_desc_k128(st + cw * (A_BYTES / 2));
+          const unsigned long long a_lo = wgmma_desc_k128(st + A_BYTES + cw * (A_BYTES / 2));
+          const unsigned long long b_hi = wgmma_desc_k128(st + C::B_OFF), b_lo = wgmma_desc_k128(st + C::B_OFF + C::B_BYTES);
+          fence_regs(acc);
+          wgmma_fence();
 #pragma unroll
-        for (int k = 0; k < BK / 8; ++k) {           // K step = 8 tf32 = 32 bytes: +2 in 16-byte units
-          const unsigned long long adv = (unsigned long long)(2 * k);
-          Wgmma<BN>::mma(acc, a_lo + adv, b_hi + adv, (in_chunk | k) != 0);
-          Wgmma<BN>::mma(acc, a_hi + adv, b_lo + adv, 1);
-          Wgmma<BN>::mma(acc, a_hi + adv, b_hi + adv, 1);
+          for (int k = 0; k < BK / 8; ++k) {         // K step = 8 tf32 = 32 bytes: +2 in 16-byte units
+            const unsigned long long adv = (unsigned long long)(2 * k);
+            Wgmma<BN>::mma(acc, a_lo + adv, b_hi + adv, (it - c0 | k) != 0);
+            Wgmma<BN>::mma(acc, a_hi + adv, b_lo + adv, 1);
+            Wgmma<BN>::mma(acc, a_hi + adv, b_hi + adv, 1);
+          }
+          wgmma_commit();
+          wgmma_wait<1>();
+          fence_regs(acc);
+          // the MMAs of the previous K block have completed: free its stage
+          __syncwarp();
+          if (pending >= 0 && lane == 0) mbar_arrive(empty(pending));
+          pending = s;
+          if (++s == C::STAGES) { s = 0; ph ^= 1u; }
         }
-        wgmma_commit();
-        if (chunk_end) wgmma_wait<0>(); else wgmma_wait<1>();
+        // chunk end: all MMAs have completed; free the last stage and add the chunk to the fp32 sum
+        wgmma_wait<0>();
         fence_regs(acc);
-        // the MMAs of the previous K block (and at a chunk end of this one) have completed: free their stages
         __syncwarp();
-        if (pending >= 0 && lane == 0) mbar_arrive(empty(pending));
-        pending = s;
-        if (chunk_end) {
-          if (lane == 0) mbar_arrive(empty(s));
-          pending = -1;
+        if (lane == 0) mbar_arrive(empty(pending));
 #pragma unroll
-          for (int c = 0; c < R; ++c) sum[c] += acc[c];
-        }
-        if (++s == C::STAGES) { s = 0; ph ^= 1u; }
+        for (int c = 0; c < R; ++c) sum[c] += acc[c];
       }
       // ---- epilogue: rows row0 and row0 + 8, columns 8j + col0 (+1) ----
 #pragma unroll

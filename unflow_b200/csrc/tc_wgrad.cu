@@ -116,7 +116,7 @@ tc_wgrad_kernel(const __grid_constant__ CUtensorMap mapP, const __grid_constant_
   auto full = [&](int s) { return bars + 8u * s; };
   auto empty = [&](int s) { return bars + 8u * (C::STAGES + s); };
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0), lane = threadIdx.x & 31;   // warp-uniform: see tc_conv.cu
   const int total_items = p.n_chunks * p.r_blocks * p.c_blocks;
 
   if (threadIdx.x == 0) {
@@ -186,43 +186,45 @@ tc_wgrad_kernel(const __grid_constant__ CUtensorMap mapP, const __grid_constant_
       const int iters = chunk_len(p, w.chunk);
 #pragma unroll
       for (int c = 0; c < R; ++c) sum[c] = 0.f;
-      int pending = -1;
-      for (int it = 0; it < iters; ++it) {
-        const int in_chunk = it % p.chunk;
-        const bool chunk_end = in_chunk == p.chunk - 1 || it == iters - 1;
-        { const long long t0 = clock64(); mbar_wait(full(s), ph); t_wait += clock64() - t0; }
-        unsigned char *stp = gbase + s * C::STAGE_BYTES;
-        split_transpose<64>(reinterpret_cast<const float *>(stp), stp + C::A_HI, stp + C::A_LO, 64 * cw, ct);
-        split_transpose<BN / 2>(reinterpret_cast<const float *>(stp + C::G_RAW), stp + C::B_HI, stp + C::B_LO,
-                                cw * (BN / 2), ct);
-        fence_proxy_async();
-        named_bar_sync(1, 256);                      // both halves of G are split
-        const unsigned st = base + s * C::STAGE_BYTES;
-        const unsigned long long a_hi = wgmma_desc_k128(st + C::A_HI + cw * (A_BYTES / 2));
-        const unsigned long long a_lo = wgmma_desc_k128(st + C::A_LO + cw * (A_BYTES / 2));
-        const unsigned long long b_hi = wgmma_desc_k128(st + C::B_HI), b_lo = wgmma_desc_k128(st + C::B_LO);
-        fence_regs(acc);
-        wgmma_fence();
+      // chunks and their K blocks as in tc_conv.cu: wait_group 1 inside a chunk, acc read only at its end
+      for (int c0 = 0; c0 < iters; c0 += p.chunk) {
+        const int c1 = c0 + p.chunk < iters ? c0 + p.chunk : iters;
+        int pending = -1;
+        for (int it = c0; it < c1; ++it) {
+          { const long long t0 = clock64(); mbar_wait(full(s), ph); t_wait += clock64() - t0; }
+          unsigned char *stp = gbase + s * C::STAGE_BYTES;
+          split_transpose<64>(reinterpret_cast<const float *>(stp), stp + C::A_HI, stp + C::A_LO, 64 * cw, ct);
+          split_transpose<BN / 2>(reinterpret_cast<const float *>(stp + C::G_RAW), stp + C::B_HI, stp + C::B_LO,
+                                  cw * (BN / 2), ct);
+          fence_proxy_async();
+          named_bar_sync(1, 256);                    // both halves of G are split
+          const unsigned st = base + s * C::STAGE_BYTES;
+          const unsigned long long a_hi = wgmma_desc_k128(st + C::A_HI + cw * (A_BYTES / 2));
+          const unsigned long long a_lo = wgmma_desc_k128(st + C::A_LO + cw * (A_BYTES / 2));
+          const unsigned long long b_hi = wgmma_desc_k128(st + C::B_HI), b_lo = wgmma_desc_k128(st + C::B_LO);
+          fence_regs(acc);
+          wgmma_fence();
 #pragma unroll
-        for (int k = 0; k < KP / 8; ++k) {
-          const unsigned long long adv = (unsigned long long)(2 * k);
-          Wgmma<BN>::mma(acc, a_lo + adv, b_hi + adv, (in_chunk | k) != 0);
-          Wgmma<BN>::mma(acc, a_hi + adv, b_lo + adv, 1);
-          Wgmma<BN>::mma(acc, a_hi + adv, b_hi + adv, 1);
+          for (int k = 0; k < KP / 8; ++k) {
+            const unsigned long long adv = (unsigned long long)(2 * k);
+            Wgmma<BN>::mma(acc, a_lo + adv, b_hi + adv, (it - c0 | k) != 0);
+            Wgmma<BN>::mma(acc, a_hi + adv, b_lo + adv, 1);
+            Wgmma<BN>::mma(acc, a_hi + adv, b_hi + adv, 1);
+          }
+          wgmma_commit();
+          wgmma_wait<1>();
+          fence_regs(acc);
+          __syncwarp();
+          if (pending >= 0 && lane == 0) mbar_arrive(empty(pending));
+          pending = s;
+          if (++s == C::STAGES) { s = 0; ph ^= 1u; }
         }
-        wgmma_commit();
-        if (chunk_end) wgmma_wait<0>(); else wgmma_wait<1>();
+        wgmma_wait<0>();
         fence_regs(acc);
         __syncwarp();
-        if (pending >= 0 && lane == 0) mbar_arrive(empty(pending));
-        pending = s;
-        if (chunk_end) {
-          if (lane == 0) mbar_arrive(empty(s));
-          pending = -1;
+        if (lane == 0) mbar_arrive(empty(pending));
 #pragma unroll
-          for (int c = 0; c < R; ++c) sum[c] += acc[c];
-        }
-        if (++s == C::STAGES) { s = 0; ph ^= 1u; }
+        for (int c = 0; c < R; ++c) sum[c] += acc[c];
       }
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
