@@ -52,7 +52,8 @@ unsigned long long unflow_launch_count(void);
 void unflow_reset_launch_count(void);
 /* Tuning knobs for tests / benchmarks.  "corr_fwd_variant": 1 (one row pair per thread) or
  * 3 (three row pairs per thread); default 1; results are bit-identical.  "tc_chunk" (1..64): K blocks per
- * tensor-core accumulation of the tc_* kernels; "tc_ksplit" (0 / 1): split the K loop of layers with few
+ * tensor-core accumulation of the tc_* kernels, default 8 (the accumulator truncates, so the error grows with
+ * the chunk: about 8x at 64); "tc_ksplit" (0 / 1): split the K loop of layers with few
  * tiles; "tc_pair_px" (0 / 1): two output-parity classes per tile in narrow transposed layers;
  * "narrow_fwd_tma" (0 / 1): TMA-staged narrow 3x3 forward. */
 int unflow_set_int_option(const char *name, int value);
@@ -292,7 +293,9 @@ int unflow_conv3x3_narrow_wgrad(const float *x, long long x_pitch, const float *
  *           (slim.conv2d; TF SAME padding enters as the offsets pad_t / pad_l, zero outside)
  *   mode 1  y[stride*iy - pad_t + ky, stride*ix - pad_l + kx] += x[iy,ix] W[ky*kw+kx]
  *           (slim.conv2d_transpose and the input gradient of mode 0; Hout, Wout % stride == 0)
- *   stride 1 or 2, kh*kw <= 64.  UNFLOW_EINVAL otherwise. */
+ *   stride 1 or 2, kh*kw <= 64.  UNFLOW_EINVAL otherwise.
+ *   Epilogue: y = act(bias + conv), or with accumulate != 0  y += act(bias + conv) (the activation applies
+ *   to this call's sum only, never to what y held before); bias may be null, act = 0 skips the activation. */
 /* Debug hook: CTA 0 of every following tc_conv launch writes its role timers
  * (clocks blocked on each pipeline barrier / in total, see csrc/tc_conv.cu) into `buf`, device memory for 16
  * long longs; nullptr switches it off. */
@@ -300,7 +303,8 @@ int unflow_tc_conv_debug(long long *buf);
 /* unflow_tc_conv_plan (host only, for the CPU tests): the tap / class / tile plan the launcher builds,
  * as integers (layout in csrc/tc_conv.cu); returns the count written, -needed when `cap` is too
  * small, -1 on invalid arguments.  mode | 4: with the two-parity-classes-per-tile rewrite the launcher applies
- * to transposed layers of 33..64 output channels. */
+ * to transposed layers of 33..64 output channels.  The last integer is the number of K slices per tile the
+ * launcher uses when the epilogue allows slicing. */
 int unflow_tc_conv_plan(int N, int Hin, int Win, int Cin, int Hout, int Wout, int Cout, int mode,
                         int stride, int kh, int kw, int pad_t, int pad_l, int *out, int cap);
 int unflow_tc_wsplit(const float *w, float *w_hi, float *w_lo, int taps, int R, int C, long long s_t,

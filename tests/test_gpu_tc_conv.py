@@ -7,6 +7,9 @@ src/e2eflow/core/flownet.py:166-233 and :89-155.
 
 Tolerance: 5e-6 of max|y| (3xTF32 split + fp32 register accumulation; measured ~1e-6, an fp32 FMA
 loop over the same K is ~2e-5 at K = 9216)."""
+import contextlib
+import ctypes
+
 import pytest
 import torch
 import torch.nn.functional as F
@@ -72,11 +75,14 @@ def test_conv_forward(N, Cin, Cout, H, W, k, stride, pads, xp, bias, act, accum)
     assert bool((obuf[..., Cout:] == -3.5).all())          # nothing written past C_out
 
 
-@pytest.mark.parametrize("bias_act,accum,dense", [(True, False, True), (False, True, False), (False, False, False)])
+@pytest.mark.parametrize("bias_act,accum,dense", [(True, False, True), (False, True, False), (False, False, False),
+                                                  (True, True, True)])
 def test_conv_k_slices(bias_act, accum, dense):
     """Few tiles, long K loop (the conv6 / conv6_1 shape of the step): the K loop of a tile is cut into slices
     on different CTAs whose partial sums meet in the output through atomics (zeroed first unless accumulating),
-    bias + leaky ReLU as a separate pass.  Same result as the float64 convolution; slack channels untouched."""
+    bias + leaky ReLU as a separate pass.  Same result as the float64 convolution; slack channels untouched.
+    Accumulating with bias + activation is y += lrelu(conv + b): the separate pass would see y_old + conv, so
+    that combination runs unsliced."""
     from unflow_b200 import _native
     t = T()
     N, Cin, Cout, H, W, k = 2, 1024, 256, 6, 20, 3
@@ -288,3 +294,203 @@ def test_launch_from_a_fresh_host_thread():
     assert result["rc"] == 0, result["err"]
     torch.cuda.synchronize()
     assert torch.equal(got, want)
+
+
+# ---------------------------------------------------------------------------------------------
+# The tuning options of unflow_set_int_option and the launch paths they select.  Every case compares one
+# launch with float64 at TOL; the plan export (unflow_tc_conv_plan) confirms the path the case is meant for.
+# ---------------------------------------------------------------------------------------------
+OPTION_DEFAULTS = {"tc_chunk": 8, "tc_pair_px": 1, "tc_ksplit": 1}
+
+
+@contextlib.contextmanager
+def options(**kv):
+    from unflow_b200 import _native
+    lib = _native.lib()
+    try:
+        for k, v in kv.items():
+            assert lib.unflow_set_int_option(k.encode(), v) == 0, (k, v)
+        yield
+    finally:
+        for k in kv:
+            lib.unflow_set_int_option(k.encode(), OPTION_DEFAULTS[k])
+
+
+def launch_plan(N, Hin, Win, Cin, Hout, Wout, Cout, mode, stride, kh, kw, pad_t, pad_l):
+    """What unflow_tc_conv does under the current options (the plan with the two-parity-classes rewrite):
+    n_classes, BN, pair_px and the K slices of a launch whose epilogue allows slicing."""
+    from unflow_b200 import _native
+    buf = (ctypes.c_int * 1024)()
+    n = _native.lib().unflow_tc_conv_plan(N, Hin, Win, Cin, Hout, Wout, Cout, mode | 4, stride, kh, kw, pad_t, pad_l,
+                                          buf, 1024)
+    assert n > 0, n
+    nt = buf[14]
+    return {"n_classes": buf[0], "tiles": buf[8] * buf[9] * buf[10], "BN": buf[12], "kblocks": buf[13], "ntaps": nt,
+            "class_start": list(buf[15:20]), "pair_px": buf[28 + 3 * nt], "ksplit": buf[n - 1]}
+
+
+def conv_case(mode, N, Cin, Cout, H, W, k, stride, pad, out_hw=None, bias=False, act=False, accum=False, yp=None,
+              seed=0):
+    """One tc_conv launch against float64.  mode 0: slim.conv2d with pad = (top, bottom, left, right); mode 1: the
+    transposed convolution with padding `pad`, cropped to out_hw.  Returns (max error / max |ref|, launch plan)."""
+    t = T()
+    x, _ = pitched(N, Cin, H, W, t.round4(Cin), seed=seed)
+    g = torch.Generator().manual_seed(seed + 1)
+    if mode == 0:
+        pt, pb, pl, pr = pad
+        w = cl((torch.randn(Cout, Cin, k, k, generator=g) * (2.0 / (Cin * k * k)) ** 0.5).cuda())
+        ref = F.conv2d(F.pad(x.double(), (pl, pr, pt, pb)), w.double(), stride=stride)
+        planes = t.split_weights(w)
+    else:
+        pt = pl = pad
+        w = cl((torch.randn(Cin, Cout, k, k, generator=g) * (2.0 / (Cin * k * k / stride ** 2)) ** 0.5).cuda())
+        Ho, Wo = (H - 1) * stride - 2 * pad + k, (W - 1) * stride - 2 * pad + k
+        oph, opw = (out_hw[0] - Ho, out_hw[1] - Wo) if out_hw else (0, 0)
+        ref = F.conv_transpose2d(x.double(), w.double(), stride=stride, padding=pad,
+                                 output_padding=(max(oph, 0), max(opw, 0)))
+        if out_hw:
+            ref = ref[:, :, :out_hw[0], :out_hw[1]]
+        planes = t.split_weights(w, transpose=True)
+    b = (torch.randn(Cout, generator=g) * 0.1).cuda() if bias else None
+    if bias:
+        ref = ref + b.double().view(1, -1, 1, 1)
+    if act:
+        ref = F.leaky_relu(ref, 0.1)
+    Ho, Wo = ref.shape[2:]
+    out, obuf = pitched(N, Cout, Ho, Wo, yp or t.round4(Cout) + 4, seed=seed + 2, fill=-3.5)
+    if accum:
+        ref = ref + out.double()
+    else:
+        out.fill_(float("nan"))
+    p = launch_plan(N, H, W, Cin, Ho, Wo, Cout, mode, stride, k, k, pt, pl)
+    t.run(x, planes, out, mode=mode, stride=stride, kh=k, kw=k, pad_t=pt, pad_l=pl, bias=b, act=act, accumulate=accum)
+    assert bool((obuf[..., Cout:] == -3.5).all())          # nothing written past C_out
+    return rel(out, ref), p
+
+
+CHUNK_FWD = [  # mode, N, Cin, Cout, H, W, k, stride, pads, bias+act: 100 and 50 K blocks per tile
+    (0, 2, 100, 96, 16, 24, 5, 1, (2, 2, 2, 2), False),      # K-sliced (3 slices at tc_chunk = 8)
+    (0, 2, 40, 50, 16, 24, 5, 2, (1, 2, 1, 2), True),
+]
+
+
+@pytest.mark.parametrize("chunk", [1, 3, 8, 64])
+@pytest.mark.parametrize("mode,N,Cin,Cout,H,W,k,stride,pads,ba", CHUNK_FWD)
+def test_chunk_option_forward(chunk, mode, N, Cin, Cout, H, W, k, stride, pads, ba):
+    """tc_chunk = K blocks per wgmma accumulation: K loops whose length is not a multiple of the chunk end in a
+    short chunk; 64 covers a whole slice in one accumulation.  Longer chunks let more truncating accumulator adds
+    pile up, so chunks past the default 8 get TOL * chunk / 8 (measured at 64 on an H100: 1.2e-5 and 6.8e-6)."""
+    with options(tc_chunk=chunk):
+        err, p = conv_case(mode, N, Cin, Cout, H, W, k, stride, pads, bias=ba, act=ba)
+    assert (p["ntaps"] * p["kblocks"]) % 3 and (p["ntaps"] * p["kblocks"]) % 8
+    assert err < TOL * max(1, chunk / 8), err
+
+
+CHUNK_WGRAD = [  # N, Cin, Cout, H, W, k, stride, pads, x pitch: 10 and 8 K blocks per work item
+    (2, 32, 96, 160, 264, 3, 1, (1, 1, 1, 1), 32),
+    (2, 70, 50, 13, 21, 3, 1, (1, 1, 1, 1), 80),
+]
+
+
+@pytest.mark.parametrize("chunk", [1, 3, 8, 64])
+@pytest.mark.parametrize("N,Cin,Cout,H,W,k,stride,pads,xp", CHUNK_WGRAD)
+def test_chunk_option_weight_gradient(chunk, N, Cin, Cout, H, W, k, stride, pads, xp):
+    with options(tc_chunk=chunk):
+        test_conv_weight_gradient(N, Cin, Cout, H, W, k, stride, pads, xp)
+
+
+PAIR = [  # mode, N, Cin, Cout, H, W, k, stride, pad, out_hw, bias+act
+    (1, 2, 130, 40, 6, 20, 4, 2, 1, None, True),              # deconvN, 40 channels: masked columns in both halves
+    (1, 2, 64, 64, 8, 12, 4, 2, 1, None, True),
+    (1, 2, 128, 64, 8, 12, 5, 2, 1, (16, 24), False),        # input gradient of 5x5 s2 SAME(1, 2)
+    (1, 2, 128, 40, 8, 12, 5, 2, 1, (16, 24), False),
+]
+
+
+@pytest.mark.parametrize("pair", [0, 1])
+@pytest.mark.parametrize("mode,N,Cin,Cout,H,W,k,stride,pad,out_hw,ba", PAIR)
+def test_pair_px_option(pair, mode, N, Cin, Cout, H, W, k, stride, pad, out_hw, ba):
+    """tc_pair_px: narrow (33..64 channel) transposed layers with two or more tiles run two output-parity classes
+    per 128-wide tile (1) or each class on its own 64-wide tile (0)."""
+    with options(tc_pair_px=pair):
+        err, p = conv_case(mode, N, Cin, Cout, H, W, k, stride, pad, out_hw=out_hw, bias=ba, act=ba, yp=Cout + 4)
+    assert p["tiles"] >= 2 and p["pair_px"] == pair and p["n_classes"] == (2 if pair else 4)
+    assert err < TOL, err
+
+
+KSPLIT = {  # mode, N, Cin, Cout, H, W, k, stride, pad, out_hw, bias+act, accumulate, y pitch
+    # input gradient of a 3x3 s1 conv6_1-like layer: 2 tiles x 2 column blocks, 288 K blocks each
+    "transposed_s1": (1, 2, 1024, 256, 6, 20, 3, 1, 1, None, False, False, 256),
+    # input gradient of a 3x3 s2 layer, one tile: its four parity classes have 4 / 2 / 2 / 1 taps, so the slices
+    # of the classes differ in length
+    "transposed_s2_3x3": (1, 2, 2048, 64, 6, 10, 3, 2, 0, (12, 20), False, False, 68),
+    # deconvN with two parity classes per tile, bias + activation as the separate pass over a dense output
+    "pair_px": (1, 2, 512, 64, 8, 12, 4, 2, 1, None, True, False, 64),
+    # the input gradient added into a channel slice of a wider buffer (a gradient slot)
+    "accumulate_pitched": (1, 2, 1024, 256, 6, 20, 3, 1, 1, None, False, True, 260),
+}
+
+
+@pytest.mark.parametrize("ksplit", [0, 1])
+@pytest.mark.parametrize("case", sorted(KSPLIT))
+def test_ksplit_option(ksplit, case):
+    """tc_ksplit: layers with few tiles and long K loops cut each tile's K loop into slices whose partial sums meet
+    in the output through atomics (1), or run one work item per tile (0)."""
+    mode, N, Cin, Cout, H, W, k, stride, pad, out_hw, ba, accum, yp = KSPLIT[case]
+    with options(tc_ksplit=ksplit):
+        err, p = conv_case(mode, N, Cin, Cout, H, W, k, stride, pad, out_hw=out_hw, bias=ba, act=ba, accum=accum,
+                           yp=yp)
+    assert (p["ksplit"] > 1) == bool(ksplit), p
+    if case == "pair_px":
+        assert p["pair_px"] == 1
+    if case == "transposed_s2_3x3":
+        cs = p["class_start"]
+        assert p["n_classes"] == 4 and [cs[i + 1] - cs[i] for i in range(4)] == [4, 2, 2, 1]
+    assert err < TOL, err
+
+
+# ---------------------------------------------------------------------------------------------
+# Same-sign operands, long K.  With U(0, 1) operands nothing cancels: |ref| is the sum of |products|, and a
+# bias in the accumulation (the truncating adds of the wgmma accumulator, see "Accuracy" in csrc/tc_conv.cu)
+# shows in full.  The error is measured elementwise, relative to each output.
+# Measured on an H100 SXM 80 GB, worst of the three layers: tc_chunk = 1: 1.1e-6, tc_chunk = 8 (the default):
+# 2.8e-6, tc_chunk = 64: 2.3e-5 -- the error grows with the chunk length as the Accuracy model predicts, and the
+# longest chunk fails SAME_SIGN_TOL (twice the worst at chunks 1 and 8).
+# ---------------------------------------------------------------------------------------------
+SAME_SIGN_TOL = 6e-6
+
+
+def same_sign_error(layer):
+    """max |got - ref| / ref of one launch at a FlowNetC shape (2B = 8 samples) with U(0, 1) operands."""
+    t = T()
+    g = torch.Generator().manual_seed(29)
+
+    def uniform(N, C, H, W, pitch):
+        buf = torch.zeros(N, H, W, pitch)
+        buf[..., :C] = torch.rand(N, H, W, C, generator=g)
+        return buf.cuda()[..., :C].permute(0, 3, 1, 2)
+
+    if layer == "conv3_1_wgrad":          # K = 8 x 48 x 160 = 61,440 pixels
+        x, gy = uniform(8, 473, 48, 160, 476), uniform(8, 256, 48, 160, 256)
+        ref = torch.nn.grad.conv2d_weight(F.pad(x.double(), (1, 1, 1, 1)), (256, 473, 3, 3), gy.double())
+        dw = cl(torch.zeros(256, 473, 3, 3, device="cuda"))
+        t.wgrad(gy, x, dw, stride=1, kh=3, kw=3, pad_t=1, pad_l=1)
+        got = dw
+    else:                                 # conv6_1: K = 9 x 1024 = 9216; conv3_1: K = 9 x 473 = 4257
+        Cin, Cout, H, W = (1024, 1024, 6, 20) if layer == "conv6_1" else (473, 256, 48, 160)
+        x = uniform(8, Cin, H, W, t.round4(Cin))
+        w = cl(torch.rand(Cout, Cin, 3, 3, generator=g).cuda())
+        ref = F.conv2d(x.double(), w.double(), padding=1)
+        got = t.empty_nhwc(8, Cout, H, W, "cuda")
+        t.run(x, t.split_weights(w), got, mode=0, stride=1, kh=3, kw=3, pad_t=1, pad_l=1)
+    assert bool((ref > 0).all())
+    return float(((got.double() - ref).abs() / ref).max())
+
+
+@pytest.mark.parametrize("chunk", [1, 8])
+@pytest.mark.parametrize("layer", ["conv6_1", "conv3_1", "conv3_1_wgrad"])
+def test_same_sign_long_k(layer, chunk):
+    with options(tc_chunk=chunk):
+        err = same_sign_error(layer)
+    print("same-sign %s tc_chunk=%d: max rel error %.3e" % (layer, chunk, err))
+    assert err <= SAME_SIGN_TOL, err

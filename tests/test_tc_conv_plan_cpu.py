@@ -26,6 +26,8 @@ def plan(N, Hin, Win, Cin, Hout, Wout, Cout, mode, stride, kh, kw, pt, pl):
     tail = v[28 + 3 * p["ntaps"]:]
     p["pair_px"] = tail[0]
     p["widx2"] = tail[1:1 + p["ntaps"]]
+    p["ksplit"] = tail[1 + p["ntaps"]]
+    assert len(tail) == 2 + p["ntaps"]
     return p
 
 
@@ -121,6 +123,37 @@ def test_plan_tiles_of_the_flownet_shapes():
         tiles = p["tiles_x"] * p["tiles_y"] * p["tiles_n"]
         util = 8 * H * W / (tiles * 128.0)
         assert util >= want - 1e-9, (H, W, p["TW"], p["TH"], p["TN"], util)
+
+
+def test_k_slices_of_the_flownet_shapes():
+    """The K-slice decision at the FlowNetC geometry (2B = 8 samples): conv6_1 (1024 -> 1024 channels, 3x3 at
+    6x20) has 8 tiles x 8 column blocks = 64 work items for 132 SMs and 288 K blocks per tile, so each tile is cut
+    into two slices; conv3 (128 -> 256 channels, 5x5 stride 2 at 48x160) fills the GPU with tiles alone.
+    tc_ksplit = 0 switches slicing off."""
+    lib = _native.lib()
+    conv6_1 = (8, 6, 20, 1024, 6, 20, 1024, 0, 1, 3, 3, 1, 1)
+    conv3 = (8, 96, 320, 128, 48, 160, 256, 0, 2, 5, 5, 1, 1)
+    assert plan(*conv6_1)["ksplit"] == 2
+    assert plan(*conv3)["ksplit"] == 1
+    try:
+        assert lib.unflow_set_int_option(b"tc_ksplit", 0) == 0
+        assert plan(*conv6_1)["ksplit"] == 1
+    finally:
+        lib.unflow_set_int_option(b"tc_ksplit", 1)
+
+
+def test_tensor_core_options_reject_values_out_of_range():
+    """unflow_set_int_option accepts tc_chunk 1..64 and tc_pair_px / tc_ksplit 0 / 1; anything else is
+    UNFLOW_EINVAL and leaves the setting alone (the plan of conv6_1 keeps its two K slices)."""
+    lib = _native.lib()
+    for name, bad in ((b"tc_chunk", 0), (b"tc_chunk", 65), (b"tc_chunk", -1), (b"tc_pair_px", 2),
+                      (b"tc_pair_px", -1), (b"tc_ksplit", 2), (b"tc_ksplit", -1)):
+        assert lib.unflow_set_int_option(name, bad) == _native.UNFLOW_EINVAL, (name, bad)
+        assert name.decode() in _native.last_error()
+    assert plan(8, 6, 20, 1024, 6, 20, 1024, 0, 1, 3, 3, 1, 1)["ksplit"] == 2
+    for name, good, default in ((b"tc_chunk", 1, 8), (b"tc_chunk", 64, 8), (b"tc_pair_px", 0, 1), (b"tc_ksplit", 0, 1)):
+        assert lib.unflow_set_int_option(name, good) == _native.UNFLOW_OK
+        assert lib.unflow_set_int_option(name, default) == _native.UNFLOW_OK
 
 
 def test_plan_rejects_bad_arguments():

@@ -529,11 +529,13 @@ extern "C" int unflow_tc_conv_debug(long long *buf) { tc::g_dbg = buf; return UN
 
 // Debug / test hook: the plan as integers --
 // [n_classes, s_in, s_out, Hit, Wit, TW, TH, TN, tiles_x, tiles_y, tiles_n, n_blocks, BN, kblocks, ntaps,
-//  class_start[5], (class_px, class_py)[4], (dx, dy, widx)[ntaps]]; returns the count written.
+//  class_start[5], (class_px, class_py)[4], (dx, dy, widx)[ntaps], pair_px, widx2[ntaps], ksplit]; returns the
+// count written.  ksplit: the K slices the launcher cuts each tile into when the epilogue allows slicing (no bias
+// and no activation, or both on a dense output that is not accumulated into), under the current tc_* options.
 extern "C" int unflow_tc_conv_plan(int N, int Hin, int Win, int Cin, int Hout, int Wout, int Cout, int mode,
                                    int stride, int kh, int kw, int pad_t, int pad_l, int *out, int cap) {
   // mode | 4: also apply the two-parity-classes-per-tile rewrite the launcher uses for narrow transposed layers
-  // (pair_px_plan); the export then ends with [pair_px, widx2[ntaps]] (the px = 1 class's tap per input offset)
+  // (pair_px_plan); pair_px = 1 then, and widx2 holds the px = 1 class's tap per input offset
   const int want_pair = (mode >> 2) & 1;
   mode &= 3;
   tc::ConvParams p{};
@@ -541,7 +543,7 @@ extern "C" int unflow_tc_conv_plan(int N, int Hin, int Win, int Cin, int Hout, i
   if (make_plan(p, BN, N, Hin, Win, Cin, Hout, Wout, Cout, mode, stride, kh, kw, pad_t, pad_l)) return -1;
   if (want_pair) pair_px_plan(p, BN, mode, stride, Cout);
   const int nt = p.class_start[p.n_classes];
-  const int need = 15 + 5 + 8 + 3 * nt + 1 + nt;
+  const int need = 15 + 5 + 8 + 3 * nt + 1 + nt + 1;
   if (!out || cap < need) return -need;
   int i = 0;
   const int head[15] = {p.n_classes, p.s_in_y, p.s_out, p.Hit, p.Wit, p.TW, p.TH, p.TN, p.tiles_x, p.tiles_y,
@@ -552,6 +554,7 @@ extern "C" int unflow_tc_conv_plan(int N, int Hin, int Win, int Cin, int Hout, i
   for (int k = 0; k < nt; ++k) { out[i++] = p.taps[k].dx; out[i++] = p.taps[k].dy; out[i++] = p.taps[k].widx; }
   out[i++] = p.pair_px;
   for (int k = 0; k < nt; ++k) out[i++] = p.taps[k].widx2;
+  out[i++] = tc::choose_ksplit(p);
   return i;
 }
 
@@ -575,9 +578,10 @@ extern "C" int unflow_tc_conv(const float *x, int N, int Hin, int Win, int Cin, 
   p.out = y; p.out_pitch = y_pitch;
   p.bias = bias; p.slope = slope; p.act = act; p.accumulate = accumulate;
   // K slices (few tiles, long K): partial sums are added into the output, which is zeroed first unless the call
-  // accumulates anyway; bias + leaky ReLU then run as unflow_bias_lrelu over the (dense) result
+  // accumulates anyway; bias + leaky ReLU then run as unflow_bias_lrelu over the (dense) result.  That pass sees
+  // only the sum in y, so a call that accumulates into y and needs it (y += act(bias + conv)) is not sliced.
   const bool post = bias && act;
-  if ((!bias && !act) || (post && y_pitch == Cout && Cout % 4 == 0)) p.ksplit = tc::choose_ksplit(p);
+  if ((!bias && !act) || (post && !accumulate && y_pitch == Cout && Cout % 4 == 0)) p.ksplit = tc::choose_ksplit(p);
   if (p.ksplit > 1 && !accumulate) {
     cudaError_t e = cudaMemset2DAsync(y, (size_t)y_pitch * 4, 0, (size_t)Cout * 4, (size_t)N * Hout * Wout, (cudaStream_t)stream);
     if (e != cudaSuccess) { set_error("tc_conv: memset of the output: %s", cudaGetErrorString(e)); return UNFLOW_ECUDA; }
