@@ -193,6 +193,36 @@ int unflow_level_loss_bwd(const float *grad_losses, const float *im1, const floa
                           int mask_occlusion, int max_distance, unsigned terms, void *stream);
 
 /* ------------------------------------------------------------------------
+ * Fused supervised flow loss of one network  (reference: supervised_loss,
+ * src/e2eflow/core/supervised.py:45-57, with charbonnier_loss losses.py:298-323):
+ *   loss = sum(mask * ((resize_bilinear(flow, [H,W]) * scale - flow_gt)^2 + 0.001^2)^0.45)
+ *          / (B*H*W*2)
+ * resize_bilinear is the legacy TF kernel (align_corners=False, no half-pixel centres):
+ * per axis src = float32(i) * float32(h/H), lo = floor(src), hi = min(ceil(src), h-1).  Any
+ * ratio h/H works (1 for full-resolution networks).  Masked elements add nothing but count in
+ * the denominator, as in the reference.
+ *   flow        [B,h,w,2] network output (network units)
+ *   flow_gt     [B,H,W,2] ground truth in pixels
+ *   mask_gt     [B,H,W,1] 0/1 validity, or NULL (every pixel valid)
+ *   loss        [1] out (device)
+ *   workspace   unflow_supervised_loss_workspace_bytes(B,H,W) bytes of scratch; one call at a
+ *               time per workspace
+ *   scale       FLOW_SCALE * 4 = 20 in the reference
+ * The sum is reduced deterministically (per-CTA partials in double, fixed-order final sum).
+ * Backward: grad_loss [1] (device) = dL/dloss -> dflow [B,h,w,2], fully written (no zeroing
+ * needed, no atomics: bit-identical across runs).  flow_gt and mask_gt carry no gradient.
+ * UNFLOW_EINVAL on a non-positive size, a tensor of 2^31 or more elements, or a NULL required
+ * pointer (everything except mask_gt).
+ * ---------------------------------------------------------------------- */
+size_t unflow_supervised_loss_workspace_bytes(int B, int H, int W);
+int unflow_supervised_loss_fwd(const float *flow, const float *flow_gt, const float *mask_gt,
+                               float *loss, void *workspace, int B, int h, int w, int H, int W,
+                               float scale, void *stream);
+int unflow_supervised_loss_bwd(const float *grad_loss, const float *flow, const float *flow_gt,
+                               const float *mask_gt, float *dflow, int B, int h, int w, int H,
+                               int W, float scale, void *stream);
+
+/* ------------------------------------------------------------------------
  * Fused Adam update on the flat parameter buffer (reference: tf.train.AdamOptimizer(beta1=0.9,
  * beta2=0.999), src/e2eflow/core/train.py:151-152; gradient averaging train.py:388-422 becomes
  * one NCCL all-reduce on `grads` before this call).  TF update rule:

@@ -21,7 +21,7 @@ def install_as_e2eflow():
     pkg = importlib.import_module("unflow_b200.e2eflow")
     sys.modules.setdefault("e2eflow", pkg)
     for sub in ("ops", "core", "core.flownet", "core.losses", "core.image_warp",
-                "core.unsupervised", "core.util"):
+                "core.unsupervised", "core.supervised", "core.util"):
         mod = importlib.import_module("unflow_b200.e2eflow." + sub)
         sys.modules.setdefault("e2eflow." + sub, mod)
     return pkg

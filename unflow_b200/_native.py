@@ -63,6 +63,9 @@ SIGNATURES = {
     "unflow_level_loss_workspace_bytes": (ctypes.c_size_t, [_i] * 3),
     "unflow_level_loss_fwd": (_i, [_vp] * 11 + [_i] * 5 + [ctypes.c_uint, _vp]),
     "unflow_level_loss_bwd": (_i, [_vp] * 11 + [_i] * 5 + [ctypes.c_uint, _vp]),
+    "unflow_supervised_loss_workspace_bytes": (ctypes.c_size_t, [_i] * 3),
+    "unflow_supervised_loss_fwd": (_i, [_vp] * 5 + [_i] * 5 + [ctypes.c_float, _vp]),
+    "unflow_supervised_loss_bwd": (_i, [_vp] * 5 + [_i] * 5 + [ctypes.c_float, _vp]),
     "unflow_conv3x3_narrow_fwd": (_i, [_vp, ctypes.c_longlong] + [_vp] * 3 + [ctypes.c_longlong] + [_i] * 5 + [_vp]),
     "unflow_conv3x3_narrow_wgrad_workspace_bytes": (ctypes.c_size_t, [_i] * 4),
     "unflow_conv3x3_narrow_wgrad": (_i, [_vp, ctypes.c_longlong, _vp] + [ctypes.c_longlong] * 4 + [_vp, _vp] + [_i] * 5 + [_vp]),

@@ -13,7 +13,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libunflow.so")
 SOURCES = ["abi.cu", "correlation.cu", "correlation_tiled.cu", "warp.cu", "forward_warp.cu",
-           "downsample.cu", "level_loss.cu", "adam.cu", "split.cu", "checksum.cu", "narrow_conv.cu", "tc_conv.cu", "tc_wgrad.cu", "relayout.cu", "narrow_conv_tma.cu"]
+           "downsample.cu", "level_loss.cu", "supervised_loss.cu", "adam.cu", "split.cu", "checksum.cu", "narrow_conv.cu", "tc_conv.cu", "tc_wgrad.cu", "relayout.cu", "narrow_conv_tma.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"]
 

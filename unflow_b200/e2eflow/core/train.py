@@ -22,6 +22,7 @@ import torch.distributed as dist
 from ... import _native
 from ..._native import check
 from .flownet import FlowNetVariables
+from .supervised import supervised_loss
 from .unsupervised import unsupervised_loss
 
 
@@ -62,10 +63,25 @@ def l2_mask_bytes(n, offsets, numels, regularised):
     return isw, (q[:, 0] | (q[:, 1] << 1) | (q[:, 2] << 2) | (q[:, 3] << 3)).contiguous()
 
 
+def _batch_and_option(args, option):
+    """Split positional arguments into the batch tensors and a trailing non-tensor option (the
+    ``lr`` of ``step(im1, im2, lr)``, the ``warmup`` of ``capture(im1, im2, warmup)``)."""
+    if args and not torch.is_tensor(args[-1]):
+        if option is not None:
+            raise TypeError("the option was given twice")
+        return tuple(args[:-1]), args[-1]
+    return tuple(args), option
+
+
 class Trainer:
     def __init__(self, params, normalization, device, variables=None, seed=1234,
-                 loss_fn=unsupervised_loss, process_group=None, augment=False):
-        """``augment``: run the reference's training-time augmentation (random_affine x3 +
+                 loss_fn=unsupervised_loss, process_group=None, augment=False, supervised=False):
+        """``supervised``: train on ``supervised_loss`` (fine-tuning on ground truth, the reference's
+        ``Trainer(..., supervised=True)``, train.py:98-112); the batch is then
+        ``(im1, im2, flow_gt, mask_gt)`` instead of ``(im1, im2)``.  ``step``, ``capture``, ``prefetch``
+        and ``step_prefetched`` take the batch tensors as positional arguments, however many there are.
+
+        ``augment``: run the reference's training-time augmentation (random_affine x3 +
         random_photometric, unsupervised.py:39-60) inside every step, as the reference Trainer does
         (``loss_fn(batch, params, normalization)`` with the default ``augment=True``,
         train.py:160,169).  run.py trains with it on; bench.py and the parity tests keep it off
@@ -81,7 +97,8 @@ class Trainer:
         self.params = dict(params)
         self.normalization = normalization
         self.device = torch.device(device)
-        self.loss_fn = loss_fn
+        self.supervised = bool(supervised)
+        self.loss_fn = supervised_loss if self.supervised else loss_fn
         self.pg = process_group
         self.world_size = dist.get_world_size(process_group) if dist.is_initialized() else 1
         spec = self.params.get('flownet', 'S')
@@ -177,8 +194,8 @@ class Trainer:
         if self.world_size > 1:
             dist.broadcast(self.flat_param, src, group=self.pg)
 
-    def loss(self, im1, im2):
-        return self.loss_fn((im1, im2), self.params, self.normalization, augment=self.augment,
+    def loss(self, *batch):
+        return self.loss_fn(tuple(batch), self.params, self.normalization, augment=self.augment,
                             variables=self.variables)
 
     def reduce_gradients(self):
@@ -270,9 +287,9 @@ class Trainer:
         torch.cuda.synchronize(self.device)
         self._hyper_lr = lr
 
-    def _step_impl(self, im1, im2):
+    def _step_impl(self, *batch):
         """forward + loss + backward + gradient mean + Adam, hyper-parameters from device memory."""
-        loss = self.loss(im1, im2)
+        loss = self.loss(*batch)
         if self.world_size > 1 and self.overlap_allreduce:
             self._backward_overlapped(loss)
         else:
@@ -287,28 +304,30 @@ class Trainer:
                 torch.cuda.current_stream().cuda_stream), "adam_step")
         return loss.detach()
 
-    def capture(self, im1, im2, warmup=3):
+    def capture(self, *batch, warmup=None):
         """Capture the whole training step (several hundred kernels: cuDNN convs, the hand-written
         kernels, the NCCL all-reduce, Adam) into ONE CUDA graph.  Later ``step`` calls copy the batch
         into the static input buffers, refresh the hyper-parameter vector and replay the graph, so
         the host launches one graph instead of ~800 kernels per step."""
+        batch, warmup = _batch_and_option(batch, warmup)
+        warmup = 3 if warmup is None else warmup
         assert self.flat_param.is_cuda
         self._hyper_dev = torch.zeros(8, device=self.device, dtype=torch.float32)
-        self._static_im1 = im1.to(self.device).clone()
-        self._static_im2 = im2.to(self.device).clone()
+        self._static = [t.to(self.device).clone() for t in batch]     # the graph's input buffers
+        self._static_im1, self._static_im2 = self._static[0], self._static[1]
         moments = (self.adam_m.clone(), self.adam_v.clone())   # restored below (resumed runs carry state)
         self._set_hyper(0.0, 1.0)                         # lr = 0 while warming up / capturing
         side = torch.cuda.Stream(device=self.device)
         side.wait_stream(torch.cuda.current_stream())
         with torch.cuda.stream(side):
             for _ in range(warmup):                       # eager warm-up (cuDNN autotune, caches)
-                self._step_impl(self._static_im1, self._static_im2)
+                self._step_impl(*self._static)
         torch.cuda.current_stream().wait_stream(side)
         torch.cuda.synchronize(self.device)
         n0 = _native.launch_count()
         graph = torch.cuda.CUDAGraph()
         with torch.cuda.graph(graph):
-            self._static_loss = self._step_impl(self._static_im1, self._static_im2)
+            self._static_loss = self._step_impl(*self._static)
         self._graph_launches = _native.launch_count() - n0
         torch.cuda.synchronize(self.device)
         # lr = 0 left the parameters alone but fed the moments: put them back, reset the step counter
@@ -319,21 +338,24 @@ class Trainer:
         return self
 
     # -- input prefetch (opt-in; graph mode) -----------------------------------------------------
-    def prefetch(self, h_im1, h_im2):
+    def prefetch(self, *host_batch):
         """Start copying the NEXT batch (pinned host tensors) into staging buffers on a copy stream;
         it overlaps the step that is currently running.  Pair with ``step_prefetched``."""
         assert self._graph is not None, "prefetch() needs a captured step (capture())"
+        if len(host_batch) != len(self._static):
+            raise ValueError("prefetch: %d tensors for a step captured with %d"
+                             % (len(host_batch), len(self._static)))
         if getattr(self, '_copy_stream', None) is None:
             self._copy_stream = torch.cuda.Stream(device=self.device)
-            self._stage_im1 = torch.empty_like(self._static_im1)
-            self._stage_im2 = torch.empty_like(self._static_im2)
+            self._stage = [torch.empty_like(t) for t in self._static]
+            self._stage_im1, self._stage_im2 = self._stage[0], self._stage[1]
             self._stage_free = None
         cs = self._copy_stream
         if self._stage_free is not None:
             cs.wait_event(self._stage_free)            # the previous contents have been consumed
         with torch.cuda.stream(cs):
-            self._stage_im1.copy_(h_im1, non_blocking=True)
-            self._stage_im2.copy_(h_im2, non_blocking=True)
+            for dst, src in zip(self._stage, host_batch):
+                dst.copy_(src, non_blocking=True)
             self._stage_ready = torch.cuda.Event()
             self._stage_ready.record(cs)
 
@@ -347,28 +369,32 @@ class Trainer:
             self._set_hyper(lr, self.iteration)
         cur = torch.cuda.current_stream(self.device)
         cur.wait_event(self._stage_ready)
-        self._static_im1.copy_(self._stage_im1, non_blocking=True)
-        self._static_im2.copy_(self._stage_im2, non_blocking=True)
+        for dst, src in zip(self._static, self._stage):
+            dst.copy_(src, non_blocking=True)
         self._stage_free = torch.cuda.Event()
         self._stage_free.record(cur)
         self._graph.replay()
         self.graph_replays += 1
         return self._static_loss
 
-    def step(self, im1, im2, lr=None):
-        """One optimisation step on this rank's shard; returns the (local) loss tensor."""
+    def step(self, *batch, lr=None):
+        """One optimisation step on this rank's shard (``step(im1, im2)``, or
+        ``step(im1, im2, flow_gt, mask_gt)`` when supervised); returns the (local) loss tensor."""
+        batch, lr = _batch_and_option(batch, lr)
         self.iteration += 1
         if lr is None:
             lr = learning_rate_at(self.iteration - 1, self.params)
         if self._graph is not None:
             if lr != self._hyper_lr:                      # the schedule moved: rewrite lr (rare)
                 self._set_hyper(lr, self.iteration)
-            self._static_im1.copy_(im1, non_blocking=True)
-            self._static_im2.copy_(im2, non_blocking=True)
+            if len(batch) != len(self._static):
+                raise ValueError("step: %d tensors for a step captured with %d" % (len(batch), len(self._static)))
+            for dst, src in zip(self._static, batch):
+                dst.copy_(src, non_blocking=True)
             self._graph.replay()
             self.graph_replays += 1
             return self._static_loss
-        loss = self.loss(im1, im2)
+        loss = self.loss(*batch)
         if self.world_size > 1 and self.overlap_allreduce:
             self._backward_overlapped(loss)
             scale = 1.0 / self.world_size

@@ -26,8 +26,15 @@
   through the reference's pairing / shuffling / resume-shift rules (core/input.py, kitti/) and
   evaluates on the KITTI 2012 training set after every ``save_interval`` chunk; each rank reads
   its own shard of the batch stream.  With ``--synthetic`` (or when [dirs] data does not exist)
-  batches are seeded synthetic pairs of the configured height x width.  Downloading the datasets
-  and the other dataset adapters (chairs, synthia, cityscapes, middlebury) are out of scope.
+  batches are seeded synthetic pairs of the configured height x width.
+* ``dataset = kitti_ft`` fine-tunes with ground truth (run.py:175-197): ``Trainer(supervised=True)``
+  on ``input_train_gt(40)`` -- KITTI 2015 + 2012 training pairs with their flow_occ ground truth,
+  the 40 held-out pairs of each set left out -- and evaluates after every ``save_interval`` chunk on
+  those 40 held-out pairs of the 2015 training set.  Parameters are [train] updated by
+  [train_kitti_ft].  With ``--synthetic`` the batches are seeded synthetic pairs with their true
+  flow and a sparse validity mask (``synthetic.supervised_batch``).
+  Downloading the datasets and the other dataset adapters (chairs, synthia, cityscapes,
+  middlebury) are out of scope.
 """
 import argparse
 import configparser
@@ -40,6 +47,7 @@ import torch
 import torch.distributed as dist
 
 KITTI_NORMALIZATION = ([104.920005, 110.1753, 114.785955], 1 / 0.0039216)  # core/input.py:45-46
+FT_HOLD_OUT = 40    # pairs of each KITTI training set kept out of the fine-tune for evaluation (run.py:187-188)
 
 
 def config_dict(config_path):
@@ -166,12 +174,27 @@ def save_checkpoint(trainer, ckpt_dir, iteration, fmt='pt'):
 def kitti_inputs(dirs, run_config, params, train_dataset, gpu_batch_size, start_iter, rank, world):
     """The 'kitti' branch of the reference run.py (:31-58, :96-115): training batches from the raw
     sequences (``input_raw(swap_images=False, center_crop=True, shift=iterations_done * batch_size)``)
-    and, when present, the KITTI 2012 training set with ground truth for evaluation at 384x1280."""
-    if train_dataset != 'kitti':
-        raise SystemExit("dataset '%s': only the KITTI input pipeline is implemented; use --synthetic"
+    and, when present, the KITTI 2012 training set with ground truth for evaluation at 384x1280.
+    The 'kitti_ft' branch (:175-197): ground-truth batches from ``input_train_gt(40)`` and, when
+    present, the KITTI 2015 training set for evaluation.  Returns (batches, eval_input)."""
+    if train_dataset not in ('kitti', 'kitti_ft'):
+        raise SystemExit("dataset '%s': only the KITTI input pipelines are implemented; use --synthetic"
                          % train_dataset)
     from .e2eflow.kitti.data import KITTIData
     from .e2eflow.kitti.input import KITTIInput
+    if train_dataset == 'kitti_ft':
+        kdata = KITTIData(dirs['data'], development=run_config.get('development', True),
+                          fast_dir=dirs.get('fast'), require=('data_scene_flow', 'data_stereo_flow'))
+        kinput = KITTIInput(data=kdata, batch_size=gpu_batch_size, normalize=False,
+                            dims=(params['height'], params['width']))
+        # batch k of the stream is fixed (file order and crop seeds), and iteration i of rank r trains on
+        # batch (i - 1) * world + r: a resumed run continues with the batches the interrupted one had
+        # not reached (the reference's queue ignores the resume shift and starts over)
+        batches = kinput.input_train_gt(FT_HOLD_OUT, rank=(start_iter - 1) * world + rank, world_size=world)
+        eval_input = None
+        if os.path.isdir(os.path.join(kdata.current_dir, 'data_scene_flow', 'training', 'flow_occ')):
+            eval_input = KITTIInput(data=kdata, batch_size=1, normalize=False, dims=(384, 1280))
+        return batches, eval_input
     kdata = KITTIData(dirs['data'], development=run_config.get('development', True),
                       fast_dir=dirs.get('fast'))
     kinput = KITTIInput(data=kdata, batch_size=gpu_batch_size, normalize=False, skipped_frames=True,
@@ -185,15 +208,17 @@ def kitti_inputs(dirs, run_config, params, train_dataset, gpu_batch_size, start_
     return batches, eval_input
 
 
-def evaluate_kitti(trainer, eval_input, device, hold_out_inv=None):
-    """train.py:265-385 on ``einput.input_train_2012()``: every pair is brought back to its file
-    size (the queue pads to 384x1280), resized bilinearly to 384x1280 for the network, and the flow
-    is resized back before AEE / outlier-% against the occluded and non-occluded ground truth."""
+def evaluate_kitti(trainer, eval_input, device, hold_out_inv=None, dataset='2012'):
+    """train.py:265-385 on ``einput.input_train_2012()`` (``dataset='2012'``) or
+    ``einput.input_train_2015()`` (``'2015'``): every pair is brought back to its file size (the
+    queue pads to 384x1280), resized bilinearly to 384x1280 for the network, and the flow is resized
+    back before AEE / outlier-% against the occluded and non-occluded ground truth."""
     from .e2eflow.core.input import resize_image_with_crop_or_pad
     from .e2eflow.core.train import evaluate
+    source = {'2012': eval_input.input_train_2012, '2015': eval_input.input_train_2015}[dataset]
 
     def examples():
-        for item in eval_input.input_train_2012(hold_out_inv):
+        for item in source(hold_out_inv):
             h, w = int(item[2][0, 0]), int(item[2][0, 1])
             yield tuple(resize_image_with_crop_or_pad(t[0], h, w).unsqueeze(0).to(device)
                         for t in (item[0], item[1]) + item[3:])
@@ -202,9 +227,12 @@ def evaluate_kitti(trainer, eval_input, device, hold_out_inv=None):
     return result
 
 
-def synthetic_batch(batch, height, width, step, rank, device):
+def synthetic_batch(batch, height, width, step, rank, device, supervised=False):
     from . import synthetic
-    im1, im2, _ = synthetic.image_pair(batch, height, width, seed=1234 + 7919 * step + rank)
+    seed = 1234 + 7919 * step + rank
+    if supervised:
+        return tuple(t.to(device) for t in synthetic.supervised_batch(batch, height, width, seed=seed))
+    im1, im2, _ = synthetic.image_pair(batch, height, width, seed=seed)
     return im1.to(device), im2.to(device)
 
 
@@ -261,7 +289,9 @@ def main(argv=None):
         dist.barrier()
 
     from .e2eflow.core.train import Trainer
-    tr = Trainer(params, KITTI_NORMALIZATION, device, seed=1234, augment=not args.no_augment)
+    supervised = train_dataset == 'kitti_ft'
+    tr = Trainer(params, KITTI_NORMALIZATION, device, seed=1234, augment=not args.no_augment,
+                 supervised=supervised)
     if tr.augment:
         from .e2eflow.core import augment as _augment
         _augment.seed(4321 + rank)      # towers / ranks differ in their augmentation draws (train.py:169)
@@ -296,19 +326,23 @@ def main(argv=None):
                                            start_iter, rank, world)
     for i in range(start_iter, num_iters + 1):
         if batches is None:
-            im1, im2 = synthetic_batch(gpu_batch_size, params['height'], params['width'], i, rank, device)
+            batch = synthetic_batch(gpu_batch_size, params['height'], params['width'], i, rank, device,
+                                    supervised=supervised)
         else:
-            im1, im2 = (t.to(device, non_blocking=True) for t in next(batches))
+            batch = tuple(t.to(device, non_blocking=True) for t in next(batches))
         if args.graph and tr._graph is None:
-            tr.capture(im1, im2)     # leaves parameters, moments and the iteration counter untouched
-        loss = tr.step(im1, im2)     # LR schedule inside (train.py:225-244)
+            tr.capture(*batch)       # leaves parameters, moments and the iteration counter untouched
+        loss = tr.step(*batch)       # LR schedule inside (train.py:225-244)
         if rank == 0 and (i == 1 or i % params['display_interval'] == 0):
             print("-- train: i = {}, loss = {}".format(i, float(loss)))
         if i % save_interval == 0:
             if not args.debug and rank == 0:
                 save_checkpoint(tr, ckpt_dir, i, args.ckpt_format)
             if eval_input is not None and rank == 0:      # Trainer.run: self.eval(1) after every chunk
-                result = evaluate_kitti(tr, eval_input, device, params.get('eval_hold_out_inv'))
+                if supervised:      # the 2015 pairs input_train_gt held out
+                    result = evaluate_kitti(tr, eval_input, device, FT_HOLD_OUT, dataset='2015')
+                else:
+                    result = evaluate_kitti(tr, eval_input, device, params.get('eval_hold_out_inv'))
                 print("-- eval: i = {}".format(i))
                 for k in sorted(result):
                     print("   {} = {}".format(k, result[k]))

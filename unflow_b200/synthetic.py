@@ -33,6 +33,20 @@ def image_pair(B, H, W, seed=1234, max_flow=8.0):
             flow.permute(0, 2, 3, 1).contiguous())
 
 
+def supervised_batch(B, H, W, seed=1234, max_flow=8.0, density=0.4):
+    """A ground-truth batch ``(im1, im2, flow_gt, mask_gt)`` like ``KITTIInput.input_train_gt``
+    delivers: float32 NHWC CPU tensors, flow in pixels [B,H,W,2], mask 0/1 [B,H,W,1].
+    ``flow_gt`` is the flow of frame 1, so ``image_warp(im2, flow_gt) ~ im1`` (``image_pair``'s flow
+    maps its second image onto its first, so its frames are swapped here).  The mask is a seeded
+    sparse set of valid pixels (``density`` of them); elsewhere the flow holds -512, what an invalid
+    KITTI ground-truth pixel (0 in the 16-bit file) decodes to."""
+    a, b, flow = image_pair(B, H, W, seed=seed, max_flow=max_flow)
+    g = torch.Generator().manual_seed(seed + 1)
+    mask = (torch.rand(B, H, W, 1, generator=g) < density).float()
+    flow_gt = torch.where(mask > 0, flow, torch.full_like(flow, -512.0))
+    return b, a, flow_gt.contiguous(), mask
+
+
 def level_inputs(B, h, w, seed=7, flow_mag=3.0):
     """Inputs of one compute_losses call: images in [0,1], smooth flows in pixels, border mask."""
     im1, im2, flow = image_pair(B, h, w, seed=seed, max_flow=flow_mag)
