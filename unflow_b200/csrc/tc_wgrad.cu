@@ -21,13 +21,15 @@
 // once (conv2: 64 channels -> two taps per block).  A chunk is a run of 32-pixel K blocks sized so that the
 // grid has a few waves of items; items of one chunk are adjacent in the schedule, so the chunk's
 // activations are read from HBM once and re-read from L2.
-//   warp 0           TMA: per K block 4 boxes of P (32 px x 32 ch each) and BN/32 boxes of G (element
-//                    stride = the conv stride, tap offset in the start coordinate, zero fill outside)
-//   warpgroups 1, 2  each splits + transposes its 64 rows of P and half of the G tile, then (after a barrier
-//                    over both, since both read all of G) issues wgmma m64nBNk8 for its 64 rows:
+//   warp 0           TMA into the raw ring: per K block 4 boxes of P (32 px x 32 ch each) and BN/32 boxes of G
+//                    (element stride = the conv stride, tap offset in the start coordinate, zero fill outside)
+//   warpgroups 1, 2  each splits + transposes its 64 rows of P and half of the G tile from a raw slot
+//                    into a split slot and frees the raw slot at once; then (after a barrier over both, since
+//                    both read all of G) issues wgmma m64nBNk8 for its 64 rows:
 //                    lo*hi + hi*lo + hi*hi per 8-pixel K step; every 8 K blocks the wgmma accumulator is
 //                    added to fp32 registers (see tc_conv.cu, "Accuracy"); at the end of the item:
-//                    red.global.add into dW
+//                    red.global.add into dW.  A warpgroup whose 64 rows all lie at or past R only splits its
+//                    half of G: no P rows, no wgmma, no epilogue.
 // dW is accumulated with fp32 atomics (split-K partial sums from several CTAs): the caller zeroes
 // it; the order of the additions, hence the last bits, vary from run to run.
 #include "tc_common.cuh"
@@ -55,20 +57,32 @@ struct WgradParams {
   long long pitch_r, pitch_t;       // dW[r * pitch_r + t * pitch_t + c]
 };
 
-// Stage: [P raw] [G raw] (TMA, unswizzled: per 32-channel group [32 px][32 ch]) and the split, transposed
-// operands [P hi] [P lo] [G hi] [G lo] (K-major, 128-byte swizzle).  Every part is a multiple of 4 KB.
+constexpr int SMEM_LIMIT = 232448;  // opt-in dynamic shared memory per block on sm_90 (227 KB)
+
+// Two rings.  Raw slot (TMA, unswizzled): [P raw] [G raw], per 32-channel group [32 px][32 ch].  Split slot
+// (consumers -> wgmma): [P hi] [P lo] [G hi] [G lo] (K-major, 128-byte swizzle).  A raw slot is free as soon as
+// both warpgroups have split it; a split slot only when the MMAs of both warpgroups on it are done.  Two split
+// slots let split(k + 1) run while MMA(k) reads the other one; the rest of shared memory holds raw slots, so
+// TMA runs several K blocks ahead of the split.  Every part is a multiple of 4 KB.
+//   BN = 128: 2 x 64 KB split + 3 x 32 KB raw;  BN = 64: 2 x 48 KB + 5 x 24 KB;  BN = 32: 2 x 40 KB + 7 x 20 KB
 template <int BN>
 struct Cfg {
   static constexpr int G_BYTES = BN * KP * 4;
-  static constexpr int G_RAW = A_BYTES;
-  static constexpr int A_HI = G_RAW + G_BYTES;
+  static constexpr int A_HI = 0;
   static constexpr int A_LO = A_HI + A_BYTES;
   static constexpr int B_HI = A_LO + A_BYTES;
   static constexpr int B_LO = B_HI + G_BYTES;
-  static constexpr int STAGE_BYTES = B_LO + G_BYTES;
-  static constexpr int STAGES = (200 * 1024 / STAGE_BYTES) < 8 ? (200 * 1024 / STAGE_BYTES) : 8;
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 + 256;
-  static_assert(STAGES >= 2, "at least two stages");
+  static constexpr int SPLIT_BYTES = B_LO + G_BYTES;
+  static constexpr int SPLIT_STAGES = 2;
+  static constexpr int G_RAW = A_BYTES;                     // within a raw slot
+  static constexpr int RAW_BYTES = A_BYTES + G_BYTES;
+  static constexpr int RAW0 = SPLIT_STAGES * SPLIT_BYTES;   // first raw slot
+  static constexpr int FIXED = RAW0 + 1024 /*alignment slack*/ + 256 /*barriers*/;
+  static constexpr int RAW_STAGES = (SMEM_LIMIT - FIXED) / RAW_BYTES < 8 ? (SMEM_LIMIT - FIXED) / RAW_BYTES : 8;
+  static constexpr int SMEM_BYTES = FIXED + RAW_STAGES * RAW_BYTES;
+  static_assert(RAW_STAGES >= 3, "TMA at least two K blocks ahead of the split");
+  static_assert(SMEM_BYTES <= SMEM_LIMIT, "over the shared memory of a block");
+  static_assert(8 * (2 * RAW_STAGES + SPLIT_STAGES) <= 256, "barriers");
 };
 
 struct Item {
@@ -112,18 +126,20 @@ tc_wgrad_kernel(const __grid_constant__ CUtensorMap mapP, const __grid_constant_
   extern __shared__ unsigned char smem_raw[];
   const unsigned base = (s32(smem_raw) + 1023u) & ~1023u;
   unsigned char *gbase = smem_raw + (base - s32(smem_raw));
-  const unsigned bars = base + C::STAGES * C::STAGE_BYTES;
-  auto full = [&](int s) { return bars + 8u * s; };
-  auto empty = [&](int s) { return bars + 8u * (C::STAGES + s); };
+  const unsigned bars = base + C::RAW0 + C::RAW_STAGES * C::RAW_BYTES;
+  auto raw_full = [&](int s) { return bars + 8u * s; };                           // raw slot s loaded
+  auto raw_empty = [&](int s) { return bars + 8u * (C::RAW_STAGES + s); };        // raw slot s split by both
+  auto split_empty = [&](int s) { return bars + 8u * (2 * C::RAW_STAGES + s); };  // MMAs of both on split slot s done
 
   const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0), lane = threadIdx.x & 31;   // warp-uniform: see tc_conv.cu
   const int total_items = p.n_chunks * p.r_blocks * p.c_blocks;
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < C::STAGES; ++s) {
-      mbar_init(full(s), 1);
-      mbar_init(empty(s), 8);          // one arrive per consumer warp
+    for (int s = 0; s < C::RAW_STAGES; ++s) {
+      mbar_init(raw_full(s), 1);
+      mbar_init(raw_empty(s), 8);      // one arrive per consumer warp
     }
+    for (int s = 0; s < C::SPLIT_STAGES; ++s) mbar_init(split_empty(s), 8);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&mapP) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&mapG) : "memory");
@@ -154,20 +170,20 @@ tc_wgrad_kernel(const __grid_constant__ CUtensorMap mapP, const __grid_constant_
         const int px = (q % p.tiles_x) * p.TW; q /= p.tiles_x;
         const int py = (q % p.tiles_y) * p.TH; q /= p.tiles_y;
         const int pn = q * p.TN;
-        { const long long t0 = clock64(); mbar_wait(empty(s), ph ^ 1u); t_wait += clock64() - t0; }
-        const unsigned st = base + s * C::STAGE_BYTES;
+        { const long long t0 = clock64(); mbar_wait(raw_empty(s), ph ^ 1u); t_wait += clock64() - t0; }
+        const unsigned st = base + C::RAW0 + s * C::RAW_BYTES;
         if (elect_one()) {
-          mbar_expect_tx(full(s), (unsigned)(A_BYTES + C::G_BYTES));
+          mbar_expect_tx(raw_full(s), (unsigned)C::RAW_BYTES);
 #pragma unroll
           for (int j = 0; j < BM / 32; ++j)       // channels past R are TMA zero fill
-            tma_4d(st + j * 4096, &mapP, full(s), w.rb * BM + 32 * j, px, py, pn);
+            tma_4d(st + j * 4096, &mapP, raw_full(s), w.rb * BM + 32 * j, px, py, pn);
 #pragma unroll
           for (int j = 0; j < GROUPS; ++j)
-            tma_4d(st + C::G_RAW + j * 4096, &mapG, full(s), gch[j], p.stride_x * px + gdx[j],
+            tma_4d(st + C::G_RAW + j * 4096, &mapG, raw_full(s), gch[j], p.stride_x * px + gdx[j],
                    p.stride * py + gdy[j], pn);
         }
         __syncwarp();
-        if (++s == C::STAGES) { s = 0; ph ^= 1u; }
+        if (++s == C::RAW_STAGES) { s = 0; ph ^= 1u; }
       }
     }
     if (p.dbg && blockIdx.x == 0 && lane == 0) { p.dbg[0] = t_wait; p.dbg[1] = clock64() - t_all; }
@@ -177,28 +193,49 @@ tc_wgrad_kernel(const __grid_constant__ CUtensorMap mapP, const __grid_constant_
     const int ct = threadIdx.x - 128 * (cw + 1);
     const int row0 = 64 * cw + 16 * (ct >> 5) + (lane >> 2);
     const int col0 = 2 * (lane & 3);
-    int s = 0;
-    unsigned ph = 0;
-    long long t_wait = 0, t_all = clock64();
+    // K blocks consumed so far: K block n uses raw slot n % RAW_STAGES and split slot n % SPLIT_STAGES (one
+    // counter instead of slot and phase registers; the BN = 128 consumer is at the 168-register limit).  The
+    // role timers are 32-bit for the same reason.
+    unsigned n = 0;
+    unsigned t_wait = 0, t_split = 0;
+    const unsigned t_all = (unsigned)clock();
+    // K block n from its raw slot into its split slot: the raw slot is released as soon as this warp has read
+    // it; the split slot is complete (both halves of G, and fenced for wgmma) after the barrier
+    auto split = [&](bool rows) {
+      const unsigned rs = n % C::RAW_STAGES, rph = (n / C::RAW_STAGES) & 1u;
+      const unsigned ss = n % C::SPLIT_STAGES, sph = (n / C::SPLIT_STAGES) & 1u;
+      { const unsigned t0 = (unsigned)clock(); mbar_wait(raw_full(rs), rph); t_wait += (unsigned)clock() - t0; }
+      { const unsigned t0 = (unsigned)clock(); mbar_wait(split_empty(ss), sph ^ 1u); t_split += (unsigned)clock() - t0; }
+      const float *raw = reinterpret_cast<const float *>(gbase + C::RAW0 + rs * C::RAW_BYTES);
+      unsigned char *sp = gbase + ss * C::SPLIT_BYTES;
+      if (rows) split_transpose<64>(raw, sp + C::A_HI, sp + C::A_LO, 64 * cw, ct);
+      split_transpose<BN / 2>(raw + C::G_RAW / 4, sp + C::B_HI, sp + C::B_LO, cw * (BN / 2), ct);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(raw_empty(rs));
+      fence_proxy_async();
+      named_bar_sync(1, 256);                        // both halves of G are split
+    };
     float sum[R], acc[R];
     for (int item = blockIdx.x; item < total_items; item += gridDim.x) {
       const Item w = decode_item(p, item);
       const int iters = chunk_len(p, w.chunk);
+      if (w.rb * BM + 64 * cw >= p.R) {
+        // all 64 rows of this warpgroup are past R: its half of G only (the other warpgroup reads it)
+        for (int it = 0; it < iters; ++it) {
+          split(false);
+          if (lane == 0) mbar_arrive(split_empty(n % C::SPLIT_STAGES));
+          ++n;
+        }
+        continue;
+      }
 #pragma unroll
       for (int c = 0; c < R; ++c) sum[c] = 0.f;
       // chunks and their K blocks as in tc_conv.cu: wait_group 1 inside a chunk, acc read only at its end
       for (int c0 = 0; c0 < iters; c0 += p.chunk) {
         const int c1 = c0 + p.chunk < iters ? c0 + p.chunk : iters;
-        int pending = -1;
         for (int it = c0; it < c1; ++it) {
-          { const long long t0 = clock64(); mbar_wait(full(s), ph); t_wait += clock64() - t0; }
-          unsigned char *stp = gbase + s * C::STAGE_BYTES;
-          split_transpose<64>(reinterpret_cast<const float *>(stp), stp + C::A_HI, stp + C::A_LO, 64 * cw, ct);
-          split_transpose<BN / 2>(reinterpret_cast<const float *>(stp + C::G_RAW), stp + C::B_HI, stp + C::B_LO,
-                                  cw * (BN / 2), ct);
-          fence_proxy_async();
-          named_bar_sync(1, 256);                    // both halves of G are split
-          const unsigned st = base + s * C::STAGE_BYTES;
+          split(true);
+          const unsigned st = base + (n % C::SPLIT_STAGES) * C::SPLIT_BYTES;
           const unsigned long long a_hi = wgmma_desc_k128(st + C::A_HI + cw * (A_BYTES / 2));
           const unsigned long long a_lo = wgmma_desc_k128(st + C::A_LO + cw * (A_BYTES / 2));
           const unsigned long long b_hi = wgmma_desc_k128(st + C::B_HI), b_lo = wgmma_desc_k128(st + C::B_LO);
@@ -215,14 +252,13 @@ tc_wgrad_kernel(const __grid_constant__ CUtensorMap mapP, const __grid_constant_
           wgmma_wait<1>();
           fence_regs(acc);
           __syncwarp();
-          if (pending >= 0 && lane == 0) mbar_arrive(empty(pending));
-          pending = s;
-          if (++s == C::STAGES) { s = 0; ph ^= 1u; }
+          if (it > c0 && lane == 0) mbar_arrive(split_empty((n - 1) % C::SPLIT_STAGES));   // MMA(n - 1) done
+          ++n;
         }
         wgmma_wait<0>();
         fence_regs(acc);
         __syncwarp();
-        if (lane == 0) mbar_arrive(empty(pending));
+        if (lane == 0) mbar_arrive(split_empty((n - 1) % C::SPLIT_STAGES));
 #pragma unroll
         for (int c = 0; c < R; ++c) sum[c] += acc[c];
       }
@@ -242,7 +278,10 @@ tc_wgrad_kernel(const __grid_constant__ CUtensorMap mapP, const __grid_constant_
         }
       }
     }
-    if (p.dbg && blockIdx.x == 0 && threadIdx.x == 128) { p.dbg[2] = t_wait; p.dbg[3] = clock64() - t_all; }
+    if (p.dbg && blockIdx.x == 0 && threadIdx.x == 128) {
+      p.dbg[2] = t_wait; p.dbg[3] = (unsigned)clock() - t_all; p.dbg[4] = t_split;
+      p.dbg[5] = C::RAW_STAGES; p.dbg[6] = C::SPLIT_STAGES;
+    }
   }
 }
 
