@@ -328,8 +328,9 @@ int unflow_conv3x3_narrow_wgrad(const float *x, long long x_pitch, const float *
  *   to this call's sum only, never to what y held before); bias may be null, act = 0 skips the activation. */
 /* Debug hook: CTA 0 of every following tc_conv launch writes its role timers
  * (clocks blocked on each pipeline barrier / in total, see csrc/tc_conv.cu) into `buf`, device memory for 16
- * long longs; nullptr switches it off.  [0, 1]: producer wait / total, [2, 3]: consumer wait / total; tc_wgrad
- * launches add [4]: consumer wait for a free split slot, [5, 6]: raw and split ring slots (csrc/tc_wgrad.cu). */
+ * long longs; nullptr switches it off.  [0, 1]: producer wait / total, [2, 3]: consumer wait / total; tc_conv
+ * launches add [5]: stages of the ring; tc_wgrad launches add [4]: consumer wait for a free split slot, [5, 6]:
+ * raw and split ring slots (csrc/tc_wgrad.cu). */
 int unflow_tc_conv_debug(long long *buf);
 /* unflow_tc_conv_plan (host only, for the CPU tests): the tap / class / tile plan the launcher builds,
  * as integers (layout in csrc/tc_conv.cu); returns the count written, -needed when `cap` is too

@@ -1,6 +1,6 @@
 // tc_conv.cu -- the conv / deconv stacks of FlowNet on the Hopper tensor cores: a wgmma implicit GEMM with
-// the 3xTF32 operand split done inside the kernel (activations: in shared memory, per K block; weights:
-// hi / lo planes made once per step).
+// the 3xTF32 operand split done inside the kernel (activations: in registers, per K step; weights: hi / lo
+// planes made once per step).
 //
 // Replaces the library convolutions behind slim.conv2d / slim.conv2d_transpose
 // (reference src/e2eflow/core/flownet.py:166-233, _flownet_upconv :89-155) for the forward pass
@@ -22,11 +22,15 @@
 //   warp 0           TMA producer: per K block one 4-D box of the ACTIVATIONS as they lie in HBM (fp32,
 //                    NHWC, any channel pitch -- e.g. a channel slice of a concat buffer; image borders,
 //                    the TF SAME padding and the channel tail are TMA zero fill, stride 2 is the tensor
-//                    map's element stride) plus the hi and lo planes of the weights, into a ring of stages.
-//   warpgroups 1, 2  consumers, 64 tile rows each: split their rows of the activation tile in shared memory
-//                    (hi = tf32(x) in place, lo = x - hi beside it), then issue wgmma m64nBNk8 kind tf32,
-//                    three per K step: lo*hi' + hi*lo' + hi*hi', fp32 accumulators in registers.  The stage
-//                    is released when the next K block's MMAs have been issued and this one's have completed.
+//                    map's element stride) plus the hi and lo planes of the weights, into a ring of stages
+//                    sized from the opt-in shared-memory limit.
+//   warpgroups 1, 2  consumers, 64 tile rows each: per K step of 8 channels each thread loads its tf32 A
+//                    fragment (4 floats) straight from the swizzled fp32 tile and splits it in registers
+//                    (hi = tf32(x), lo = x - hi), then the warpgroup issues wgmma m64nBNk8 kind tf32 with A
+//                    from registers, three per K step: lo*hi' + hi*lo' + hi*hi', fp32 accumulators in
+//                    registers.  One wgmma group per K step; two fragment sets alternate, so a K step's MMAs
+//                    run while the next one's fragment is loaded.  The stage is released once the next K
+//                    block's first group has been issued and every group of this one has completed.
 //                    The K loop is cut into CHUNKS of 8 K blocks (tc_common.cuh: CHUNK): every chunk starts a
 //                    fresh wgmma accumulator that is then added to a second fp32 register accumulator with
 //                    round to nearest (see "Accuracy"); after the last chunk: bias + leaky ReLU (or += for
@@ -79,16 +83,27 @@ struct ConvParams {
   Tap taps[MAX_TAPS];
 };
 
-// Stage: [A raw -> hi after the split] [A lo] [B hi] [B lo].  Each 1024-byte aligned (128-byte swizzle atoms).
+// Stage: [A raw fp32] [B hi] [B lo].  Each 1024-byte aligned (128-byte swizzle atoms).  The ring fills the opt-in
+// limit: BN = 128: 4 x 48 KB, BN = 64: 7 x 32 KB, BN = 32: 8 x 24 KB (capped at 8).
 template <int BN>
 struct Cfg {
   static constexpr int B_BYTES = BN * BK * 4;
-  static constexpr int STAGE_BYTES = 2 * A_BYTES + 2 * B_BYTES;
-  static constexpr int B_OFF = 2 * A_BYTES;
-  static constexpr int STAGES = (200 * 1024 / STAGE_BYTES) < 8 ? (200 * 1024 / STAGE_BYTES) : 8;
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*alignment slack*/ + 256 /*barriers*/;
+  static constexpr int STAGE_BYTES = A_BYTES + 2 * B_BYTES;
+  static constexpr int B_OFF = A_BYTES;
+  static constexpr int FIXED = 1024 /*alignment slack*/ + 256 /*barriers*/;
+  static constexpr int STAGES = (SMEM_LIMIT - FIXED) / STAGE_BYTES < 8 ? (SMEM_LIMIT - FIXED) / STAGE_BYTES : 8;
+  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + FIXED;
   static_assert(STAGES >= 2, "at least two stages");
+  static_assert(SMEM_BYTES <= SMEM_LIMIT, "over the shared memory of a block");
 };
+// Fragment sets of the consumer (hi + lo tf32 A fragments of one K step each): K step k of a K block uses set
+// k % FRAG_SETS and is one wgmma group, so a set is rewritten once wait_group FRAG_SETS - 1 has retired the group
+// that read it.  Two sets divide the 4 K steps of a block, keep the set index a compile-time constant and leave
+// the MMAs of one K step in flight while the next one's fragment is loaded and split.  Four sets compile as
+// cleanly but were not faster (DESIGN.md §3.8).  After the wait of K step FRAG_SETS - 1, only groups of the
+// current K block can still run: that is where the previous block's stage is released.
+constexpr int FRAG_SETS = 2;
+static_assert((BK / 8) % FRAG_SETS == 0 && FRAG_SETS <= BK / 8, "fragment sets per K block");
 
 struct TileCoord {
   int cls, n0, iy0, ix0, nb;
@@ -159,6 +174,9 @@ tc_conv_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
   }
   __syncthreads();
 
+  // registers: 40 for warpgroup 0, 232 for the consumers (40 * 128 + 232 * 256 <= 64K).  Each setmaxnreg sits
+  // inside its role's branch: ptxas ignores one in code shared by both roles (C7507).
+  if (warp < 4) setmaxnreg_dec<40>();
   if (warp == 0) {
     // ===================== TMA producer (whole warp converged, one elected lane issues) =====================
     int s = 0;
@@ -195,64 +213,62 @@ tc_conv_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
     }
     if (p.dbg && blockIdx.x == 0 && lane == 0) { p.dbg[0] = t_wait; p.dbg[1] = clock64() - t_all; }
   } else if (warp >= 4) {
-    // ===================== consumers: split, wgmma, epilogue =====================
+    // ===================== consumers: A fragments, split, wgmma, epilogue =====================
+    setmaxnreg_inc<232>();
     const int cw = (warp >> 2) - 1;                  // consumer warpgroup: tile rows [64 cw, 64 cw + 64)
     const int ct = threadIdx.x - 128 * (cw + 1);     // thread within the warpgroup
-    const int row0 = 64 * cw + 16 * (ct >> 5) + (lane >> 2);     // this thread's accumulator rows: row0, row0 + 8
+    const int row0 = 64 * cw + 16 * (ct >> 5) + (lane >> 2);     // this thread's accumulator / A rows: row0, row0 + 8
     const int col0 = 2 * (lane & 3);
     const int per_img = p.TW * p.TH;
     int s = 0;
     unsigned ph = 0;
     long long t_wait = 0, t_all = clock64();
     float sum[R], acc[R];
+    unsigned a_hi[FRAG_SETS][4], a_lo[FRAG_SETS][4];
     for (int item = blockIdx.x; item < total_items; item += gridDim.x) {
       const Work wk = decode_work(p, item);
       const TileCoord t = wk.t;
       const int iters = wk.iters;
 #pragma unroll
       for (int c = 0; c < R; ++c) sum[c] = 0.f;
-      // Outer loop over chunks, inner loop over the K blocks of a chunk.  The inner loop only ever waits for the
-      // previous K block's MMAs (wait_group 1), so they overlap this block's split; the accumulator is read only
-      // after the inner loop, behind wait_group 0.  A read of acc inside the inner loop would make ptxas wait for
-      // every MMA group (C7517).
+      // Outer loop over chunks, inner loop over the K blocks of a chunk.  Inside a chunk the only waits are
+      // wait_group FRAG_SETS - 1 before a fragment set is rewritten, so the MMAs run while the next K step's
+      // fragment is loaded and split; the accumulator is read only after the inner loop, behind wait_group 0.
+      // A read of acc inside the inner loop would make ptxas wait for every MMA group (C7517).
       for (int c0 = 0; c0 < iters; c0 += p.chunk) {
         const int c1 = c0 + p.chunk < iters ? c0 + p.chunk : iters;
         int pending = -1;                            // stage whose MMAs may still be running
         for (int it = c0; it < c1; ++it) {
           { const long long t0 = clock64(); mbar_wait(full(s), ph); t_wait += clock64() - t0; }
-          // split this warpgroup's 64 rows (8 KB): the elementwise split keeps the swizzled positions
-          {
-            float4 *a = reinterpret_cast<float4 *>(gbase + s * C::STAGE_BYTES + cw * (A_BYTES / 2));
-            float4 *l = reinterpret_cast<float4 *>(gbase + s * C::STAGE_BYTES + A_BYTES + cw * (A_BYTES / 2));
-#pragma unroll
-            for (int j = 0; j < A_BYTES / 2 / 16 / 128; ++j) {
-              const int i = ct + 128 * j;
-              const float4 v = a[i], h = tf32_hi4(v);
-              a[i] = h;
-              l[i] = sub4(v, h);
-            }
-          }
-          fence_proxy_async();                       // generic-proxy writes -> visible to the tensor core
-          named_bar_sync(1 + cw, 128);
+          const float *a = reinterpret_cast<const float *>(gbase + s * C::STAGE_BYTES);
           const unsigned st = base + s * C::STAGE_BYTES;
-          const unsigned long long a_hi = wgmma_desc_k128(st + cw * (A_BYTES / 2));
-          const unsigned long long a_lo = wgmma_desc_k128(st + A_BYTES + cw * (A_BYTES / 2));
           const unsigned long long b_hi = wgmma_desc_k128(st + C::B_OFF), b_lo = wgmma_desc_k128(st + C::B_OFF + C::B_BYTES);
-          fence_regs(acc);
-          wgmma_fence();
 #pragma unroll
           for (int k = 0; k < BK / 8; ++k) {         // K step = 8 tf32 = 32 bytes: +2 in 16-byte units
+            unsigned (&hi)[4] = a_hi[k % FRAG_SETS], (&lo)[4] = a_lo[k % FRAG_SETS];
+            wgmma_wait<FRAG_SETS - 1>();             // the group that last read this set has completed
+            fence_regs(acc);
+            if (k == FRAG_SETS - 1) {
+              // every group of the previous K block has completed: free its stage
+              __syncwarp();
+              if (pending >= 0 && lane == 0) mbar_arrive(empty(pending));
+            }
+            // this thread's tf32 A fragment of the K step, straight from the swizzled fp32 tile (the 8 rows of a
+            // quarter-warp lie in 8 different 16-byte chunks: no bank conflicts), split in registers
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {
+              const float x = a[sw128_offset(row0 + 8 * (e & 1), 8 * k + (lane & 3) + 4 * (e >> 1)) / 4];
+              const float h = tf32_rna_fast(x);
+              hi[e] = __float_as_uint(h);
+              lo[e] = __float_as_uint(x - h);
+            }
+            wgmma_fence();
             const unsigned long long adv = (unsigned long long)(2 * k);
-            Wgmma<BN>::mma(acc, a_lo + adv, b_hi + adv, (it - c0 | k) != 0);
-            Wgmma<BN>::mma(acc, a_hi + adv, b_lo + adv, 1);
-            Wgmma<BN>::mma(acc, a_hi + adv, b_hi + adv, 1);
+            Wgmma<BN>::mma_rs(acc, lo, b_hi + adv, (it - c0 | k) != 0);
+            Wgmma<BN>::mma_rs(acc, hi, b_lo + adv, 1);
+            Wgmma<BN>::mma_rs(acc, hi, b_hi + adv, 1);
+            wgmma_commit();
           }
-          wgmma_commit();
-          wgmma_wait<1>();
-          fence_regs(acc);
-          // the MMAs of the previous K block have completed: free its stage
-          __syncwarp();
-          if (pending >= 0 && lane == 0) mbar_arrive(empty(pending));
           pending = s;
           if (++s == C::STAGES) { s = 0; ph ^= 1u; }
         }
@@ -310,7 +326,9 @@ tc_conv_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
         }
       }
     }
-    if (p.dbg && blockIdx.x == 0 && threadIdx.x == 128) { p.dbg[2] = t_wait; p.dbg[3] = clock64() - t_all; }
+    if (p.dbg && blockIdx.x == 0 && threadIdx.x == 128) {
+      p.dbg[2] = t_wait; p.dbg[3] = clock64() - t_all; p.dbg[5] = C::STAGES;
+    }
   }
 }
 
@@ -524,7 +542,7 @@ static bool pair_px_plan(tc::ConvParams &p, int &BN, int mode, int stride, int C
 
 // Debug hook: role timers.  `buf` = device memory for 16 long longs (or nullptr to switch off); every following
 // tc_conv launch makes CTA 0 write, in clocks: [0] TMA producer blocked on a free stage, [1] its total; [2] the
-// first consumer thread blocked on the TMA data, [3] its total.
+// first consumer thread blocked on the TMA data, [3] its total, [5] the stages of the ring.
 extern "C" int unflow_tc_conv_debug(long long *buf) { tc::g_dbg = buf; return UNFLOW_OK; }
 
 // Debug / test hook: the plan as integers --

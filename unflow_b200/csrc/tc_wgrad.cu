@@ -57,8 +57,6 @@ struct WgradParams {
   long long pitch_r, pitch_t;       // dW[r * pitch_r + t * pitch_t + c]
 };
 
-constexpr int SMEM_LIMIT = 232448;  // opt-in dynamic shared memory per block on sm_90 (227 KB)
-
 // Two rings.  Raw slot (TMA, unswizzled): [P raw] [G raw], per 32-channel group [32 px][32 ch].  Split slot
 // (consumers -> wgmma): [P hi] [P lo] [G hi] [G lo] (K-major, 128-byte swizzle).  A raw slot is free as soon as
 // both warpgroups have split it; a split slot only when the MMAs of both warpgroups on it are done.  Two split
