@@ -15,7 +15,11 @@ Python and is what decides WHICH frames are trained on.  That logic is kept verb
   k pairs of a ``random.seed(0)`` shuffle.
 
 Instead of TF queues a batch iterator with a small prefetch thread decodes PNGs (OpenCV) into
-pinned host tensors ``[B,H,W,3]`` float32 in [0,255], RGB like ``tf.image.decode_png``.
+pinned host tensors ``[B,H,W,3]`` float32 in [0,255], RGB like ``tf.image.decode_png``; with
+``num_threads`` > 1 the pairs of a batch are decoded on a pool of that many threads, into the same
+slots with the same crop seeds (bit-identical batches).
+* ``sequence_pairs`` / ``sequence_files`` (sintel/input.py, middlebury/input.py): per sorted
+  sequence directory frame k paired with frame k + 1, and the sorted per-sequence ground-truth lists.
 With ``rank`` / ``world_size`` each rank takes every world_size-th batch: distinct shards per GPU
 (the reference's towers all dequeue the same batch, SURVEY.md R4).
 """
@@ -90,9 +94,10 @@ def resize_output_flow(t, height, width, channels=2):
 class _Prefetcher:
     """Iterator over ``make(i)`` for i = first, first+step, ... produced by a daemon thread."""
 
-    def __init__(self, make, first, step, depth=4):
+    def __init__(self, make, first, step, depth=4, pool=None):
         self._q = queue.Queue(maxsize=depth)
         self._stop = threading.Event()
+        self._pool = pool
 
         def work():
             i = first
@@ -127,6 +132,8 @@ class _Prefetcher:
 
     def close(self):
         self._stop.set()
+        if self._pool is not None:
+            self._pool.shutdown(wait=False)
 
 
 class Input():
@@ -156,6 +163,24 @@ class Input():
         if self.normalize:
             image = self._normalize_image(image)
         return image
+
+    def _decode_pool(self):
+        """A pool of ``num_threads`` decode threads ([run] num_input_threads; OpenCV releases the GIL),
+        None for one thread."""
+        if self.num_threads <= 1:
+            return None
+        from concurrent.futures import ThreadPoolExecutor
+        return ThreadPoolExecutor(self.num_threads, thread_name_prefix='decode')
+
+    @staticmethod
+    def _fill(pool, load, n):
+        """``load(k)`` for k < n: in order on the calling thread, or spread over ``pool``.  Each
+        ``load`` writes only its own slot k of the batch, so both give the same batch."""
+        if pool is None:
+            for k in range(n):
+                load(k)
+        else:
+            list(pool.map(load, range(n)))
 
     # -- which files ---------------------------------------------------------------------------
     def raw_pairs(self, swap_images=True, sequence=True, shift=0, seed=0, skip=0):
@@ -207,6 +232,36 @@ class Input():
             pairs = pairs[:hold_out_inv]
         return pairs
 
+    def sequence_pairs(self, image_dir, exclude=()):
+        """Per sorted sub-directory of ``image_dir`` (one sequence each), frame k paired with frame
+        k + 1 (sintel/input.py:63-84, middlebury/input.py:66-87); sub-directories named in
+        ``exclude`` are skipped."""
+        image_dir = os.path.join(self.data.current_dir, image_dir)
+        pairs = []
+        for sub_name in sorted(os.listdir(image_dir)):
+            if sub_name in exclude:
+                continue
+            sub_dir = os.path.join(image_dir, sub_name)
+            files = sorted(os.listdir(sub_dir))
+            pairs += [(os.path.join(sub_dir, files[i]), os.path.join(sub_dir, files[i + 1]))
+                      for i in range(len(files) - 1)]
+        return pairs
+
+    def _input_sequence_test(self, image_dir, exclude=()):
+        """``_input_test`` over ``sequence_pairs``: ``(im1, im2, input_shape)``, batch 1."""
+        for fn1, fn2 in self.sequence_pairs(image_dir, exclude):
+            raw1, raw2 = read_png_image(fn1), read_png_image(fn2)
+            yield (self._preprocess_image(raw1).unsqueeze(0), self._preprocess_image(raw2).unsqueeze(0),
+                   torch.tensor(raw1.shape).unsqueeze(0))
+
+    def _preprocess_truth(self, t):
+        """A ground-truth map [h,w,c] -> [1,H,W,c] cropped / padded to ``dims`` (``_preprocess_flow``)."""
+        height, width = self.dims
+        t = torch.as_tensor(t).float()
+        if t.dim() == 2:
+            t = t.unsqueeze(-1)
+        return resize_image_with_crop_or_pad(t, height, width).unsqueeze(0)
+
     # -- batches -------------------------------------------------------------------------------
     def input_raw(self, swap_images=True, sequence=True,
                   needs_crop=True, shift=0, seed=0,
@@ -218,25 +273,32 @@ class Input():
         B = self.batch_size
         pin = torch.cuda.is_available() if pin is None else pin
 
+        pool = self._decode_pool()
+
         def make(batch_index):
             gen = torch.Generator().manual_seed(crop_seed * 1000003 + batch_index)
+            # the crop seeds of the whole batch are drawn first, in order, so they do not depend on
+            # which thread decodes which pair
+            seeds = [int(torch.randint(0, 2 ** 31 - 1, (1,), generator=gen)) for _ in range(B)] if needs_crop else None
             a = torch.empty((B, height, width, 3), dtype=torch.float32, pin_memory=pin)
             b = torch.empty((B, height, width, 3), dtype=torch.float32, pin_memory=pin)
-            for k in range(B):
+
+            def load(k):
                 fn1, fn2 = pairs[(batch_index * B + k) % len(pairs)]
                 im1, im2 = read_png_image(fn1), read_png_image(fn2)
                 if needs_crop:
-                    s = int(torch.randint(0, 2 ** 31 - 1, (1,), generator=gen))
-                    im1, im2 = augment.random_crop([im1, im2], [height, width, 3], seed=s)
+                    im1, im2 = augment.random_crop([im1, im2], [height, width, 3], seed=seeds[k])
                 else:
                     im1, im2 = im1.reshape(height, width, 3), im2.reshape(height, width, 3)
                 if self.normalize:
                     im1, im2 = self._normalize_image(im1), self._normalize_image(im2)
                 a[k].copy_(im1)
                 b[k].copy_(im2)
+
+            self._fill(pool, load, B)
             return a, b
 
-        return _Prefetcher(make, rank, world_size)
+        return _Prefetcher(make, rank, world_size, pool=pool)
 
     def _input_test(self, image_dir, hold_out_inv=None):
         """One pass over the pairs of ``image_dir``: ``(im1, im2, input_shape)`` with batch 1
@@ -245,3 +307,16 @@ class Input():
             raw1, raw2 = read_png_image(fn1), read_png_image(fn2)
             yield (self._preprocess_image(raw1).unsqueeze(0), self._preprocess_image(raw2).unsqueeze(0),
                    torch.tensor(raw1.shape).unsqueeze(0))
+
+
+def sequence_files(parent_dir, ignore_last=False):
+    """sintel/input.py:38-49 ``_get_filenames``: the sorted files of every sorted sub-directory,
+    each sub-directory's last file dropped with ``ignore_last``."""
+    filenames = []
+    for sub_name in sorted(os.listdir(parent_dir)):
+        sub_dir = os.path.join(parent_dir, sub_name)
+        files = sorted(os.listdir(sub_dir))
+        if ignore_last:
+            files = files[:-1]
+        filenames += [os.path.join(sub_dir, f) for f in files]
+    return filenames

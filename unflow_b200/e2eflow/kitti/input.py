@@ -101,20 +101,25 @@ class KITTIInput(Input):
         B = self.batch_size
         pin = torch.cuda.is_available() if pin is None else pin
 
+        pool = self._decode_pool()
+
         def make(batch_index):
             gen = torch.Generator().manual_seed(crop_seed * 1000003 + batch_index)
+            seeds = [int(torch.randint(0, 2 ** 31 - 1, (1,), generator=gen)) for _ in range(B)]
             out = [torch.empty((B, height, width, c), dtype=torch.float32, pin_memory=pin) for c in (3, 3, 2, 1)]
-            for k in range(B):
+
+            def load(k):
                 fn1, fn2, fn_gt = triples[(batch_index * B + k) % len(triples)]
                 im1, im2 = read_png_image(fn1), read_png_image(fn2)
                 flow, mask = read_kitti_flow(fn_gt)
                 gt = torch.cat([torch.as_tensor(flow), torch.as_tensor(mask)], 2).float()
-                s = int(torch.randint(0, 2 ** 31 - 1, (1,), generator=gen))
-                im1, im2, gt = augment.random_crop([im1, im2, gt], [height, width, 3], seed=s)
+                im1, im2, gt = augment.random_crop([im1, im2, gt], [height, width, 3], seed=seeds[k])
                 if self.normalize:
                     im1, im2 = self._normalize_image(im1), self._normalize_image(im2)
                 for dst, src in zip(out, (im1, im2, gt[:, :, 0:2], gt[:, :, 2:3])):
                     dst[k].copy_(src)
+
+            self._fill(pool, load, B)
             return tuple(out)
 
-        return _Prefetcher(make, rank, world_size)
+        return _Prefetcher(make, rank, world_size, pool=pool)

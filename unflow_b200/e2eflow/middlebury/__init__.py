@@ -1,0 +1,1 @@
+"""Middlebury data directories and inputs (reference src/e2eflow/middlebury/)."""

@@ -3,11 +3,17 @@ non-interactive part of the reference's ``eval_gui.py`` (src/eval_gui.py:96-352)
 
     python -m unflow_b200.eval --dataset kitti --variant train_2012 --ex my_experiment --num 10
     python -m unflow_b200.eval --variant test_2015 --ex C,CSS --num -1 --output_benchmark
+    python -m unflow_b200.eval --dataset sintel --variant train_final --ex C --num -1
+
+Datasets and variants: kitti (train_2012, train_2015, test_2012, test_2015), chairs (test),
+sintel (train_clean, train_final, test_clean, test_final), mdb (train, test); with ``--num -1``
+the Sintel test variants evaluate 552 pairs and Middlebury test 12, as the reference does.
 
 For every experiment in ``--ex`` the newest checkpoint is looked up under [dirs] log /ex/<name>, then
 [dirs] checkpoints/<name> (eval_gui.py:100-108; TensorFlow checkpoints of the reference and this
 implementation's ``.pt`` files are both accepted), the networks are restored, and every example is
-run at the input's fixed size (KITTI: 384x1280): ``resize_input`` -> ``unsupervised_loss(...,
+run at the dataset's fixed size (KITTI 384x1280, FlyingChairs 384x512, Sintel 512x1024,
+Middlebury 512x640): ``resize_input`` -> ``unsupervised_loss(...,
 augment=False, return_flow=True)`` -> ``resize_output_flow`` back to the file size.  Printed per
 experiment: ``EPE_noc, EPE_all, outliers_noc, outliers_all`` (eval_gui.py:175-178), or ``EPE_all`` /
 nothing for variants with other / no ground truth.  ``--output_benchmark`` writes
@@ -27,6 +33,46 @@ import torch
 from .run import config_dict, convert_input_strings, latest_checkpoint
 
 KITTI_VARIANTS = ('train_2012', 'train_2015', 'test_2012', 'test_2015')
+# dataset -> (variants, network input height x width) (eval_gui.py:298-322)
+DATASETS = {'kitti': (KITTI_VARIANTS, (384, 1280)),
+            'chairs': (('test',), (384, 512)),
+            'sintel': (('train_clean', 'train_final', 'test_clean', 'test_final'), (512, 1024)),
+            'mdb': (('train', 'test'), (512, 640))}
+# pairs evaluated with --num -1 where the reference sets a number (eval_gui.py:315-322)
+ALL_PAIRS = {('sintel', 'test_clean'): 552, ('sintel', 'test_final'): 552, ('mdb', 'test'): 12}
+
+
+def check_variant(dataset, variant):
+    if dataset not in DATASETS:
+        raise SystemExit("--dataset %s: must be one of %s" % (dataset, ', '.join(DATASETS)))
+    if variant not in DATASETS[dataset][0]:
+        raise SystemExit("--variant %s: %s has %s" % (variant, dataset, ', '.join(DATASETS[dataset][0])))
+
+
+def dataset_input(dataset, variant, data_dir):
+    """The input object of ``dataset`` at its network size (batch 1, unnormalised) and the iterator of
+    ``variant``: ``(im1, im2, input_shape[, ground truth])`` per pair."""
+    check_variant(dataset, variant)
+    dims = DATASETS[dataset][1]
+    if dataset == 'kitti':
+        from .e2eflow.kitti.data import KITTIData
+        from .e2eflow.kitti.input import KITTIInput
+        need = 'data_stereo_flow' if variant.endswith('2012') else 'data_scene_flow'
+        data_input = KITTIInput(KITTIData(data_dir, development=True, require=(need,)), batch_size=1,
+                                normalize=False, dims=dims)
+    elif dataset == 'chairs':
+        from .e2eflow.chairs.data import ChairsData
+        from .e2eflow.chairs.input import ChairsInput
+        data_input = ChairsInput(ChairsData(data_dir), batch_size=1, normalize=False, dims=dims)
+    elif dataset == 'sintel':
+        from .e2eflow.sintel.data import SintelData
+        from .e2eflow.sintel.input import SintelInput
+        data_input = SintelInput(SintelData(data_dir), batch_size=1, normalize=False, dims=dims)
+    else:
+        from .e2eflow.middlebury.data import MiddleburyData
+        from .e2eflow.middlebury.input import MiddleburyInput
+        data_input = MiddleburyInput(MiddleburyData(data_dir), batch_size=1, normalize=False, dims=dims)
+    return data_input, getattr(data_input, 'input_' + variant)
 
 
 def flow_to_int16(flow):
@@ -149,8 +195,9 @@ def experiment_setup(name, default_config_path, dataset):
 
 def main(argv=None):
     ap = argparse.ArgumentParser()
-    ap.add_argument('--dataset', default='kitti', help='only kitti is implemented')
-    ap.add_argument('--variant', default='train_2012', choices=KITTI_VARIANTS)
+    ap.add_argument('--dataset', default='kitti', choices=tuple(DATASETS))
+    ap.add_argument('--variant', default='train_2012',
+                    help='; '.join('%s: %s' % (d, ', '.join(v)) for d, (v, _) in DATASETS.items()))
     ap.add_argument('--ex', default='', help='Experiment name(s) (can be comma separated list).')
     ap.add_argument('--num', type=int, default=10, help='Number of examples to evaluate. -1 = all.')
     ap.add_argument('--gpu', default='0')
@@ -162,8 +209,7 @@ def main(argv=None):
     ap.add_argument('--config', default=os.environ.get('UNFLOW_CONFIG', '../config.ini'))
     ap.add_argument('--out', default='../out')
     args = ap.parse_args(argv)
-    if args.dataset != 'kitti':
-        raise SystemExit("dataset '%s': only kitti is implemented" % args.dataset)
+    check_variant(args.dataset, args.variant)
     if not torch.cuda.is_available():
         raise SystemExit("unflow_b200.eval needs a CUDA device (no CPU fallback)")
     device = torch.device('cuda', int(args.gpu.split(',')[0]))
@@ -177,13 +223,12 @@ def run_eval(args, device, make_flow_fn=network_flow_fn):
     print("-- evaluating: on {} pairs from {}/{}".format(args.num, args.dataset, args.variant))
 
     from .e2eflow.core.flownet import FlowNetVariables
-    from .e2eflow.kitti.data import KITTIData
-    from .e2eflow.kitti.input import KITTIInput
     from .run import restore_checkpoint
     dirs = config_dict(args.config)['dirs']
-    need = 'data_stereo_flow' if args.variant.endswith('2012') else 'data_scene_flow'
-    data = KITTIData(dirs['data'], development=True, require=(need,))
-    data_input = KITTIInput(data, batch_size=1, normalize=False, dims=(384, 1280))
+    data_input, input_fn = dataset_input(args.dataset, args.variant, dirs['data'])
+    num = args.num
+    if num == -1:
+        num = ALL_PAIRS.get((args.dataset, args.variant), num)
     results = {}
     for name in [n for n in args.ex.split(',') if n]:
         params, ckpt, config_path = experiment_setup(name, args.config, args.dataset)
@@ -201,10 +246,9 @@ def run_eval(args, device, make_flow_fn=network_flow_fn):
                 shutil.rmtree(out_dir)
             os.makedirs(out_dir)
             shutil.copyfile(config_path, os.path.join(out_dir, 'config.ini'))
-        items = getattr(data_input, 'input_' + args.variant)()
         results[name] = evaluate_examples(
-            name, items, data_input.dims, make_flow_fn(params, data_input.get_normalization(), variables),
-            device, num=args.num, out_dir=out_dir, output_benchmark=args.output_benchmark,
+            name, input_fn(), data_input.dims, make_flow_fn(params, data_input.get_normalization(), variables),
+            device, num=num, out_dir=out_dir, output_benchmark=args.output_benchmark,
             output_visual=args.output_visual, output_backward=args.output_backward, output_png=args.output_png)
     return results
 

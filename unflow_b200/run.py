@@ -33,8 +33,14 @@
   those 40 held-out pairs of the 2015 training set.  Parameters are [train] updated by
   [train_kitti_ft].  With ``--synthetic`` the batches are seeded synthetic pairs with their true
   flow and a sparse validity mask (``synthetic.supervised_batch``).
-  Downloading the datasets and the other dataset adapters (chairs, synthia, cityscapes,
-  middlebury) are out of scope.
+* ``dataset = chairs | synthia | cityscapes`` trains unsupervised on FlyingChairs (unrelated 384x512
+  pairs of ``flying_chairs/image``, converted from the release layout when needed), the SYNTHIA
+  sequences (consecutive frames, random crop) or the Cityscapes sequences (frame distances 1 and 2,
+  random crop) with the reference's arguments (run.py:62-173, ``dataset_inputs``), and like
+  ``kitti`` evaluates on the KITTI 2012 training set after every chunk when it is under [dirs] data.
+  [run] num_input_threads threads decode the pairs of a batch (bit-identical batches for any count).
+  With ``--synthetic`` every dataset trains on seeded synthetic pairs of its height x width.
+  Datasets are never downloaded: a missing directory is an error naming the expected layout.
 """
 import argparse
 import configparser
@@ -178,15 +184,15 @@ def kitti_inputs(dirs, run_config, params, train_dataset, gpu_batch_size, start_
     The 'kitti_ft' branch (:175-197): ground-truth batches from ``input_train_gt(40)`` and, when
     present, the KITTI 2015 training set for evaluation.  Returns (batches, eval_input)."""
     if train_dataset not in ('kitti', 'kitti_ft'):
-        raise SystemExit("dataset '%s': only the KITTI input pipelines are implemented; use --synthetic"
-                         % train_dataset)
+        raise SystemExit("dataset '%s': kitti_inputs serves kitti and kitti_ft (dataset_inputs dispatches "
+                         "the others)" % train_dataset)
     from .e2eflow.kitti.data import KITTIData
     from .e2eflow.kitti.input import KITTIInput
     if train_dataset == 'kitti_ft':
         kdata = KITTIData(dirs['data'], development=run_config.get('development', True),
                           fast_dir=dirs.get('fast'), require=('data_scene_flow', 'data_stereo_flow'))
         kinput = KITTIInput(data=kdata, batch_size=gpu_batch_size, normalize=False,
-                            dims=(params['height'], params['width']))
+                            dims=(params['height'], params['width']), num_threads=run_config.get('num_input_threads', 1))
         # batch k of the stream is fixed (file order and crop seeds), and iteration i of rank r trains on
         # batch (i - 1) * world + r: a resumed run continues with the batches the interrupted one had
         # not reached (the reference's queue ignores the resume shift and starts over)
@@ -198,10 +204,53 @@ def kitti_inputs(dirs, run_config, params, train_dataset, gpu_batch_size, start_
     kdata = KITTIData(dirs['data'], development=run_config.get('development', True),
                       fast_dir=dirs.get('fast'))
     kinput = KITTIInput(data=kdata, batch_size=gpu_batch_size, normalize=False, skipped_frames=True,
-                        dims=(params['height'], params['width']))
+                        dims=(params['height'], params['width']), num_threads=run_config.get('num_input_threads', 1))
     batches = kinput.input_raw(swap_images=False, center_crop=True,
                                shift=(start_iter - 1) * run_config['batch_size'],
                                rank=rank, world_size=world)
+    eval_input = None
+    if os.path.isdir(os.path.join(kdata.current_dir, 'data_stereo_flow', 'training', 'flow_occ')):
+        eval_input = KITTIInput(data=kdata, batch_size=1, normalize=False, dims=(384, 1280))
+    return batches, eval_input
+
+
+def dataset_inputs(dirs, run_config, params, train_dataset, gpu_batch_size, start_iter, rank, world):
+    """The dataset branches of the reference run.py (:62-202): training batches of ``train_dataset``
+    and the KITTI 2012 training set (at 384x1280) the run evaluates on after every chunk, or None when
+    that set is not under [dirs] data.  kitti / kitti_ft: ``kitti_inputs``.
+
+    * chairs: ``ChairsInput.input_raw(swap_images=False, shift=...)`` -- unrelated 384x512 pairs, no crop;
+    * synthia: ``KITTIInput(SynthiaData).input_raw(swap_images=False, shift=...)`` -- consecutive frames of
+      every sequence / view, random crop, no ``skipped_frames``;
+    * cityscapes: ``KITTIInput(CityscapesData, skipped_frames=False).input_raw(swap_images=False,
+      center_crop=True, skip=[0, 1], shift=...)`` -- ``center_crop`` is a no-op in the reference, which
+      random-crops, and the pairs that span two snippets of a city directory are kept, as there.
+
+    ``shift`` is the reference's resume shift (iterations done x [run] batch_size); each rank reads its
+    own shard of the batch stream; [run] num_input_threads threads decode a batch."""
+    if train_dataset in ('kitti', 'kitti_ft'):
+        return kitti_inputs(dirs, run_config, params, train_dataset, gpu_batch_size, start_iter, rank, world)
+    from .e2eflow.kitti.input import KITTIInput
+    kw = dict(batch_size=gpu_batch_size, normalize=False, dims=(params['height'], params['width']),
+              num_threads=run_config.get('num_input_threads', 1))
+    data_kw = dict(development=run_config.get('development', True), fast_dir=dirs.get('fast'))
+    stream = dict(swap_images=False, shift=(start_iter - 1) * run_config['batch_size'], rank=rank, world_size=world)
+    if train_dataset == 'chairs':
+        from .e2eflow.chairs.data import ChairsData
+        from .e2eflow.chairs.input import ChairsInput
+        batches = ChairsInput(ChairsData(dirs['data'], **data_kw), **kw).input_raw(**stream)
+    elif train_dataset == 'synthia':
+        from .e2eflow.synthia.data import SynthiaData
+        batches = KITTIInput(SynthiaData(dirs['data'], **data_kw), **kw).input_raw(**stream)
+    elif train_dataset == 'cityscapes':
+        from .e2eflow.cityscapes.data import CityscapesData
+        batches = KITTIInput(CityscapesData(dirs['data'], **data_kw), skipped_frames=False,
+                             **kw).input_raw(center_crop=True, skip=[0, 1], **stream)
+    else:
+        raise SystemExit("dataset '%s': must be one of synthia, kitti, kitti_ft, cityscapes, chairs"
+                         % train_dataset)
+    from .e2eflow.kitti.data import KITTIData
+    kdata = KITTIData(dirs['data'], fast_dir=dirs.get('fast'), require=())
     eval_input = None
     if os.path.isdir(os.path.join(kdata.current_dir, 'data_stereo_flow', 'training', 'flow_occ')):
         eval_input = KITTIInput(data=kdata, batch_size=1, normalize=False, dims=(384, 1280))
@@ -322,8 +371,8 @@ def main(argv=None):
     batches, eval_input = None, None
     data_dir = dirs.get('data', '')
     if not args.synthetic and os.path.isdir(data_dir):
-        batches, eval_input = kitti_inputs(dirs, run_config, params, train_dataset, gpu_batch_size,
-                                           start_iter, rank, world)
+        batches, eval_input = dataset_inputs(dirs, run_config, params, train_dataset, gpu_batch_size,
+                                             start_iter, rank, world)
     for i in range(start_iter, num_iters + 1):
         if batches is None:
             batch = synthetic_batch(gpu_batch_size, params['height'], params['width'], i, rank, device,
