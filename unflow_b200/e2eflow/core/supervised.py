@@ -21,7 +21,7 @@ from ..._native import check
 from . import tf_image
 from .flownet import FLOW_SCALE, flownet, get_variables
 from .losses import charbonnier_loss
-from .unsupervised import _device_constant, _track_loss
+from .unsupervised import _clear_tracked, _device_constant, _track_image, _track_loss
 
 
 def fused_available(flow, flow_gt):
@@ -90,7 +90,15 @@ def flow_loss(flow, flow_gt, mask_gt=None, scale=FLOW_SCALE * 4, fused=None):
     return charbonnier_loss(final - flow_gt, mask_gt)
 
 
+def _final_flow(flow, size):
+    """The network's finest flow in pixels at the ground truth's size (reference :51-54)."""
+    if tuple(flow.shape[1:3]) == tuple(size):
+        return flow * (FLOW_SCALE * 4)
+    return tf_image.resize_bilinear(flow, size) * (FLOW_SCALE * 4)
+
+
 def supervised_loss(batch, params, normalization=None, augment=True, variables=None):
+    _clear_tracked()
     im1, im2, flow_gt, mask_gt = batch
     im1 = im1 / 255.0
     im2 = im2 / 255.0
@@ -103,6 +111,12 @@ def supervised_loss(batch, params, normalization=None, augment=True, variables=N
             brightness_stddev=0.02, min_colour=0.9, max_colour=1.1, min_gamma=0.7, max_gamma=1.5)
     else:
         im1_photo, im2_photo = im1, im2
+    # reference :27-30; the colour images are made from the tracked tensors when a summary is written
+    from .flow_util import flow_to_color
+    _track_image(im1_photo, 'im1_photo')
+    _track_image(im2_photo, 'im2_photo')
+    _track_image(flow_gt, 'flow_gt', flow_to_color)
+    _track_image(mask_gt, 'mask_gt')
 
     spec = params.get('flownet', 'S')
     full_res = params.get('full_res')
@@ -118,6 +132,8 @@ def supervised_loss(batch, params, normalization=None, augment=True, variables=N
     for i, net_flows in enumerate(reversed(flows_fw)):
         # the last network of a full_res stack predicts at full resolution: a ratio-1 "resize"
         net_loss = flow_loss(net_flows[0], flow_gt, mask_gt, scale=FLOW_SCALE * 4)
+        _track_image(net_flows[0], 'flow_pred_' + str(i),
+                     lambda f, size=tuple(flow_gt.shape[1:3]): flow_to_color(_final_flow(f, size)))
         final_loss = final_loss + net_loss / (2 ** i)
 
     regularization_loss = variables.regularization_loss()

@@ -124,6 +124,8 @@ class Trainer:
         self._flatten()
         self.iteration = 0
         self._graph = None
+        # keep the tracked images of every step for image summaries (unsupervised.tracked_images)
+        self.track_images = False
         # L2 regularisation gradient inside the Adam kernel (CUDA only; UNFLOW_L2_IN_ADAM=0: autograd forms it).
         # flat_grad then holds the gradient of the data terms only -- l2_gradient() is the missing part.
         self.l2_mask = None
@@ -195,6 +197,8 @@ class Trainer:
             dist.broadcast(self.flat_param, src, group=self.pg)
 
     def loss(self, *batch):
+        from . import unsupervised
+        unsupervised.track_images = self.track_images
         return self.loss_fn(tuple(batch), self.params, self.normalization, augment=self.augment,
                             variables=self.variables)
 
@@ -329,6 +333,10 @@ class Trainer:
         with torch.cuda.graph(graph):
             self._static_loss = self._step_impl(*self._static)
         self._graph_launches = _native.launch_count() - n0
+        # the tracked values of the captured step live in the graph's memory: every replay rewrites them
+        from . import unsupervised
+        self._graph_tracked = (dict(unsupervised.tracked), dict(unsupervised.tracked_params),
+                               dict(unsupervised.tracked_images))
         torch.cuda.synchronize(self.device)
         # lr = 0 left the parameters alone but fed the moments: put them back, reset the step counter
         self.adam_m.copy_(moments[0]); self.adam_v.copy_(moments[1]); self.flat_grad.zero_()
@@ -404,8 +412,32 @@ class Trainer:
         self.apply_update(lr, scale)
         return loss.detach()
 
+    def tracked(self):
+        """The last step's tracked values as (losses, params, images): {op name: tensor or float} in
+        the order the reference creates the ops, {op name: float} and {op name: (tensor, to_image)}.
+        After ``capture`` these are the captured step's outputs, which every replay refreshes."""
+        if self._graph is not None:
+            return self._graph_tracked
+        from . import unsupervised
+        return unsupervised.tracked, unsupervised.tracked_params, unsupervised.tracked_images
 
-def evaluate(variables, params, normalization, examples, eval_size=(384, 1280)):
+    def summary_scalars(self):
+        """{op name: float} of the last step's tracked losses, read with one device-to-host copy."""
+        return read_scalars(self.tracked()[0])
+
+
+def read_scalars(values):
+    """{name: float} of a dict of scalar tensors and Python numbers; the tensors are stacked on their
+    device and copied to the host at once."""
+    names = [k for k, v in values.items() if torch.is_tensor(v)]
+    out = {k: float(v) for k, v in values.items() if not torch.is_tensor(v)}
+    if names:
+        host = torch.stack([values[k].reshape(()).float() for k in names]).cpu()
+        out.update(zip(names, host.tolist()))
+    return {k: out[k] for k in values}
+
+
+def evaluate(variables, params, normalization, examples, eval_size=(384, 1280), loss_averages=None):
     """The checkpoint-evaluation loop of the reference Trainer (train.py:265-385) without the TF
     session / summary scaffolding.
 
@@ -415,13 +447,15 @@ def evaluate(variables, params, normalization, examples, eval_size=(384, 1280)):
     run through ``unsupervised_loss(augment=False, return_flow=True)``, the flow is resized back and
     rescaled (``resize_output_flow``), and AEE / outlier-% are averaged over the examples for the
     'occluded' (all valid) and 'non-occluded' masks (train.py:314-321).  Returns the dict of
-    averages plus the last example's visualisation tensors (train.py:290-293)."""
+    averages plus the last example's visualisation tensors (train.py:290-293).  ``loss_averages``: a
+    dict that receives every tracked loss of ``unsupervised_loss`` averaged over the examples
+    (train.py:323-328), {op name: float}."""
     from . import flow_util, tf_image
     from .flow_io import resize_output_flow
     from .image_warp import image_warp
     from .losses import DISOCC_THRESH, create_outgoing_mask, occlusion
     from ..ops import forward_warp
-    sums, n, images = {}, 0, None
+    sums, loss_sums, n, images = {}, {}, 0, None
     rh, rw = eval_size
     with torch.no_grad():
         for (im1, im2, flow_occ, mask_occ, flow_noc, mask_noc) in examples:
@@ -430,6 +464,10 @@ def evaluate(variables, params, normalization, examples, eval_size=(384, 1280)):
             b = tf_image.resize_bilinear(im2, [rh, rw])
             _, flow, flow_bw = unsupervised_loss((a, b), params, normalization, augment=False,
                                                  return_flow=True, variables=variables)
+            if loss_averages is not None:
+                from .unsupervised import tracked
+                for k, v in read_scalars(tracked).items():
+                    loss_sums[k] = loss_sums.get(k, 0.0) + v
             flow = resize_output_flow(flow, h, w).contiguous()
             flow_bw = resize_output_flow(flow_bw, h, w).contiguous()
             for name, gt, mask in (('occluded', flow_occ, mask_occ), ('non-occluded', flow_noc, mask_noc)):
@@ -444,4 +482,6 @@ def evaluate(variables, params, normalization, examples, eval_size=(384, 1280)):
                       'flow error': flow_util.flow_error_image(flow, flow_occ, mask_occ, mask_noc)}
     out = {k: v / max(n, 1) for k, v in sums.items()}
     out['num_examples'] = n
+    if loss_averages is not None:
+        loss_averages.update({k: v / max(n, 1) for k, v in loss_sums.items()})
     return out, images

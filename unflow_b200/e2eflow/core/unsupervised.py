@@ -31,14 +31,32 @@ _LEVEL_DISTANCES = [3, 2, 2, 1, 1]
 _FULL_RES_WEIGHTS = [12.7, 5.5, 5.0, 4.35, 3.9, 3.4, 1.1]
 _FULL_RES_DISTANCES = [3, 3] + _LEVEL_DISTANCES
 
-# TF collects tracked scalars in graph collections (_track_loss, reference :18-19); the eager
-# counterpart is a dict refreshed on every call.
+# TF collects tracked values in graph collections (reference :18-24, :158-159); the eager counterparts
+# are dicts refilled on every call, keyed by the reference's op names ('loss2/ternary', 'loss/combined',
+# 'weight/ternary', 'train/augmented1') in the order TF creates the ops.  ``tracked_images`` is filled
+# only while ``track_images`` is set (core/train.py sets it when image summaries are written): it keeps
+# the tracked batches alive until the next call.  Its values are ``(tensor, to_image)``, the callable
+# turning the tensor into the summarised image when a summary is written (None: the tensor itself).
 tracked = {}
+tracked_params = {}
+tracked_images = {}
+track_images = False
 _const_cache = {}
 
 
 def _track_loss(op, name):
     tracked[name] = op.detach() if torch.is_tensor(op) else op
+
+
+def _track_image(op, name, to_image=None):
+    if track_images:
+        tracked_images['train/' + name] = (op.detach(), to_image)
+
+
+def _clear_tracked():
+    tracked.clear()
+    tracked_params.clear()
+    tracked_images.clear()
 
 
 def _device_constant(values, device):
@@ -67,6 +85,7 @@ def _augmented(frame1, frame2, border_mask):
 
 def unsupervised_loss(batch, params, normalization=None, augment=True,
                       return_flow=False, variables=None):
+    _clear_tracked()
     frame1, frame2 = (f / 255.0 for f in batch)
     size = frame1.shape[1:3]
     mean = _device_constant([m / 255.0 for m in normalization[0]], frame1.device)
@@ -75,6 +94,8 @@ def unsupervised_loss(batch, params, normalization=None, augment=True,
     # the loss compares images in [0, 1]; the network sees mean-subtracted (and jittered) copies
     if augment:
         loss_im1, loss_im2, net_im1, net_im2, border_mask = _augmented(frame1, frame2, border_mask)
+        _track_image(net_im1, 'augmented1')
+        _track_image(net_im2, 'augmented2')
     else:
         loss_im1, loss_im2, net_im1, net_im2 = frame1, frame2, frame1, frame2
 
@@ -113,6 +134,7 @@ def unsupervised_loss(batch, params, normalization=None, augment=True,
     per_vec = None
     total = 0.0
     for lvl in range(n_levels):
+        scope = 'loss%d/' % (lvl + 2)                      # the level's variable scope (reference :117-121)
         to_pixels = top_scale / (2 ** lvl)                 # network units -> pixels at this level
         terms = compute_losses(level_im1, level_im2,
                                pyramid_fw[lvl] * to_pixels, pyramid_bw[lvl] * to_pixels,
@@ -126,7 +148,7 @@ def unsupervised_loss(batch, params, normalization=None, augment=True,
             # scalar multiply + add per term and level (about 100 one-element kernels per step and as many
             # again in the backward pass); same sum, order of the fp32 additions aside
             for t in active:
-                _track_loss(terms[t], t)
+                _track_loss(terms[t], scope + t)
             wvec = _device_constant([(params.get(t + '_weight') or 0.0) if t in active else 0.0
                                      for t in fused_loss.TERM_ORDER], vec.device)
             level_sum = torch.dot(vec, wvec)
@@ -134,7 +156,7 @@ def unsupervised_loss(batch, params, normalization=None, augment=True,
         else:
             level_sum = 0.0
             for t in active:
-                _track_loss(terms[t], t)
+                _track_loss(terms[t], scope + t)
                 level_sum = level_sum + params[t + '_weight'] * terms[t]
                 per_term[t] = per_term[t] + weights[lvl] * terms[t]
         total = total + weights[lvl] * level_sum
@@ -151,6 +173,8 @@ def unsupervised_loss(batch, params, normalization=None, augment=True,
     _track_loss(final_loss, 'loss/combined')
     for t in LOSSES:
         _track_loss(per_term[t], 'loss/' + t)
+        if params.get(t + '_weight'):
+            tracked_params['weight/' + t] = params[t + '_weight']
 
     if return_flow:
         return final_loss, final_flow(pyramid_fw[0]), final_flow(pyramid_bw[0])

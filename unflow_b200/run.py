@@ -41,6 +41,13 @@
   [run] num_input_threads threads decode the pairs of a batch (bit-identical batches for any count).
   With ``--synthetic`` every dataset trains on seeded synthetic pairs of its height x width.
   Datasets are never downloaded: a missing directory is an error naming the expected layout.
+* TensorBoard summaries (train.py:66-86,187-261,314-370; experiment.py:14-25), from rank 0 only, also
+  with ``--debug``: ``<[dirs] log>/ex/<name>/train`` gets the learning rate, every tracked loss and the
+  weights of the weighted terms at i = 1 and every ``display_interval`` steps (the steps the loss is
+  printed at); with ``--debug`` also the tracked images, as the reference adds image summaries in debug
+  mode only.  ``<[dirs] log>/ex/<name>/eval`` gets the AEE / outlier averages and every tracked loss
+  averaged over the evaluation set after every ``save_interval`` chunk, at that iteration.  ``--ow``
+  removes both.  View them with ``tensorboard --logdir <[dirs] log>/ex``.
 """
 import argparse
 import configparser
@@ -257,11 +264,12 @@ def dataset_inputs(dirs, run_config, params, train_dataset, gpu_batch_size, star
     return batches, eval_input
 
 
-def evaluate_kitti(trainer, eval_input, device, hold_out_inv=None, dataset='2012'):
+def evaluate_kitti(trainer, eval_input, device, hold_out_inv=None, dataset='2012', loss_averages=None):
     """train.py:265-385 on ``einput.input_train_2012()`` (``dataset='2012'``) or
     ``einput.input_train_2015()`` (``'2015'``): every pair is brought back to its file size (the
     queue pads to 384x1280), resized bilinearly to 384x1280 for the network, and the flow is resized
-    back before AEE / outlier-% against the occluded and non-occluded ground truth."""
+    back before AEE / outlier-% against the occluded and non-occluded ground truth.  ``loss_averages``:
+    a dict that receives the tracked losses averaged over the pairs (core/train.py: evaluate)."""
     from .e2eflow.core.input import resize_image_with_crop_or_pad
     from .e2eflow.core.train import evaluate
     source = {'2012': eval_input.input_train_2012, '2015': eval_input.input_train_2015}[dataset]
@@ -272,8 +280,51 @@ def evaluate_kitti(trainer, eval_input, device, hold_out_inv=None, dataset='2012
             yield tuple(resize_image_with_crop_or_pad(t[0], h, w).unsqueeze(0).to(device)
                         for t in (item[0], item[1]) + item[3:])
 
-    result, _ = evaluate(trainer.variables, trainer.params, trainer.normalization, examples())
+    result, _ = evaluate(trainer.variables, trainer.params, trainer.normalization, examples(),
+                         loss_averages=loss_averages)
     return result
+
+
+def summary_writers(log_dir, name, rank, overwrite=False):
+    """The train and eval event-file writers of experiment ``name`` (experiment.py:14-25), on rank 0
+    only (None, None elsewhere).  ``overwrite`` (``--ow``) removes the earlier runs' files first."""
+    if rank != 0:
+        return None, None
+    from .e2eflow.core.summary import SummaryWriter
+    dirs = [os.path.join(log_dir, 'ex', name, d) for d in ('train', 'eval')]
+    if overwrite:
+        for d in dirs:
+            if os.path.isdir(d):
+                shutil.rmtree(d)
+    return tuple(SummaryWriter(d) for d in dirs)
+
+
+def write_train_summaries(writer, trainer, step, lr, images=False):
+    """train.py:253-255 at a display step: the learning rate, the tracked losses (one device-to-host
+    copy) and the weights under the reference's tags; with ``images`` the tracked images too."""
+    from .e2eflow.core import summary
+    from .e2eflow.core.train import read_scalars
+    losses, params, tracked_images = trainer.tracked()
+    tags = summary.train_tags(losses, params, tracked_images if images else ())
+    writer.scalar(tags['learning_rate']['learning_rate'], lr, step)
+    for kind, values in (('losses', read_scalars(losses)), ('params', params)):
+        for name, value in values.items():
+            writer.scalar(tags[kind][name], value, step)
+    if images:
+        for name, (t, to_image) in tracked_images.items():
+            writer.image(tags['images'][name], to_image(t) if to_image is not None else t, step)
+    writer.flush()
+
+
+def write_eval_summaries(writer, step, result, loss_averages):
+    """train.py:365-370: the evaluation averages under the reference's eval tags."""
+    from .e2eflow.core import summary
+    tags = summary.eval_tags(loss_averages)
+    for name in summary.EVAL_METRICS:
+        writer.scalar(tags[name], result[name], step)
+    for name, value in loss_averages.items():
+        writer.scalar(tags[summary.strip_tower(name)], value, step)
+    writer.flush()
 
 
 def synthetic_batch(batch, height, width, step, rank, device, supervised=False):
@@ -334,13 +385,16 @@ def main(argv=None):
             os.makedirs(ex_dir, exist_ok=True)
             if args.ow or not os.path.isfile(os.path.join(ex_dir, 'config.ini')):
                 shutil.copyfile(args.config, os.path.join(ex_dir, 'config.ini'))
+    # before any step: without the tensorboard package the run stops here
+    train_writer, eval_writer = summary_writers(log_dir, args.ex, rank, overwrite=args.ow)
     if world > 1:
         dist.barrier()
 
-    from .e2eflow.core.train import Trainer
+    from .e2eflow.core.train import Trainer, learning_rate_at
     supervised = train_dataset == 'kitti_ft'
     tr = Trainer(params, KITTI_NORMALIZATION, device, seed=1234, augment=not args.no_augment,
                  supervised=supervised)
+    tr.track_images = args.debug and train_writer is not None      # train.py:156
     if tr.augment:
         from .e2eflow.core import augment as _augment
         _augment.seed(4321 + rank)      # towers / ranks differ in their augmentation draws (train.py:169)
@@ -363,6 +417,9 @@ def main(argv=None):
         restore_checkpoint(tr, source[1], nets=[i])
     if start_iter > num_iters:
         print('-- train: max_iter reached')
+        for w in (train_writer, eval_writer):
+            if w is not None:
+                w.close()
         return
     tr.broadcast_variables(0)
     if rank == 0:
@@ -384,23 +441,31 @@ def main(argv=None):
         loss = tr.step(*batch)       # LR schedule inside (train.py:225-244)
         if rank == 0 and (i == 1 or i % params['display_interval'] == 0):
             print("-- train: i = {}, loss = {}".format(i, float(loss)))
+            write_train_summaries(train_writer, tr, i, learning_rate_at(i - 1, params), images=tr.track_images)
         if i % save_interval == 0:
             if not args.debug and rank == 0:
                 save_checkpoint(tr, ckpt_dir, i, args.ckpt_format)
             if eval_input is not None and rank == 0:      # Trainer.run: self.eval(1) after every chunk
+                loss_averages = {}
                 if supervised:      # the 2015 pairs input_train_gt held out
-                    result = evaluate_kitti(tr, eval_input, device, FT_HOLD_OUT, dataset='2015')
+                    result = evaluate_kitti(tr, eval_input, device, FT_HOLD_OUT, dataset='2015',
+                                            loss_averages=loss_averages)
                 else:
-                    result = evaluate_kitti(tr, eval_input, device, params.get('eval_hold_out_inv'))
+                    result = evaluate_kitti(tr, eval_input, device, params.get('eval_hold_out_inv'),
+                                            loss_averages=loss_averages)
                 print("-- eval: i = {}".format(i))
                 for k in sorted(result):
                     print("   {} = {}".format(k, result[k]))
+                write_eval_summaries(eval_writer, i, result, loss_averages)
             if world > 1:
                 # rank 0 alone writes the checkpoint and evaluates: the others wait here instead of inside the
                 # next step's all-reduce (where the wait would run into the NCCL watchdog and count as step time)
                 dist.barrier()
     if batches is not None:
         batches.close()
+    for w in (train_writer, eval_writer):
+        if w is not None:
+            w.close()
     if world > 1:
         if args.graph:
             # ncclCommDestroy was observed to hang for minutes when the communicator had been used
