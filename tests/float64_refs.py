@@ -116,6 +116,14 @@ def _fp32_sum(grid, f):
     return f + (s - f).detach()
 
 
+def _fp32_frac(f, fl):
+    """f - floor(f) rounded to fp32, differentiable w.r.t. f (float64).  image_warp defines its bilinear weights
+    by this fp32 difference (reference image_warp.py:26-27): a flow a hair below an integer has a fraction within
+    an ulp of 1, whose rounding is a large relative error of the other side's weight 1 - fraction."""
+    s = (f.detach().float() - fl.float()).double()
+    return (f - fl) + (s - (f - fl)).detach()
+
+
 def warp_taps(flow, mode):
     """Tap pixels and bilinear weights of one gather: mode 0 = BackwardWarp (zero outside), 1 = image_warp
     (clamped taps), 2 = spatial transformer (absolute coordinates, weights from the clamped taps).  Returns
@@ -132,7 +140,7 @@ def warp_taps(flow, mode):
         x, y = _fp32_sum(gx, u), _fp32_sum(gy, v)
     if mode == 1:
         fu, fv = torch.floor(u).detach(), torch.floor(v).detach()
-        xw, yw = u - fu, v - fv
+        xw, yw = _fp32_frac(u, fu), _fp32_frac(v, fv)
         x0, y0 = gx + fu.long(), gy + fv.long()
     else:
         x0, y0 = torch.floor(x).detach().long(), torch.floor(y).detach().long()
@@ -154,11 +162,13 @@ def warp_taps(flow, mode):
     return [(cy0, cx0, wl * wt, ones), (cy1, cx0, wl * yb, ones), (cy0, cx1, xr * wt, ones), (cy1, cx1, xr * yb, ones)]
 
 
-def warp(img, flow, mode):
-    """The bilinear gather of unflow_backward_warp_fwd in float64 (differentiable w.r.t. img and flow)."""
+def warp(img, flow, mode, skip_tap=None):
+    """The bilinear gather of unflow_backward_warp_fwd in float64 (differentiable w.r.t. img and flow).
+    `skip_tap`: leave tap t of warp_taps out (a wrong kernel, for the negative control)."""
     out = 0
-    for yy, xx, wgt, valid in warp_taps(flow, mode):
-        out = out + (wgt * valid)[..., None] * _gather(img, yy, xx)
+    for t, (yy, xx, wgt, valid) in enumerate(warp_taps(flow, mode)):
+        if t != skip_tap:
+            out = out + (wgt * valid)[..., None] * _gather(img, yy, xx)
     return out
 
 
@@ -171,10 +181,10 @@ def warp_abs(img, flow, mode):
 
 
 @torch.enable_grad()        # also inside a backward pass, where autograd is off
-def warp_grads(grad, img, flow, mode):
-    """(dimage, dflow) of sum(grad * warp(img, flow)) by float64 autograd, and their A."""
+def warp_grads(grad, img, flow, mode, skip_tap=None):
+    """(dimage, dflow) of sum(grad * warp(img, flow)) by float64 autograd, and their A (of the full warp)."""
     i, f = img.detach().requires_grad_(True), flow.detach().requires_grad_(True)
-    dimg, dflow = torch.autograd.grad((warp(i, f, mode) * grad).sum(), (i, f))
+    dimg, dflow = torch.autograd.grad((warp(i, f, mode, skip_tap) * grad).sum(), (i, f))
     B, H, W, C = img.shape
     f = flow.detach()
     taps = warp_taps(f, mode)
@@ -476,3 +486,28 @@ def level_loss_grad_scale(L, mfw, mbw, gl):
                 Aout[:, y0 + ey:y1 + ey, x0 + ex:x1 + ex] += k
                 Aout[:, y0:y1, x0:x1] += 2 * k
     return Af, Ab
+
+
+# ---- the fused supervised flow loss (csrc/supervised_loss.cu; reference supervised.py:45-57) ---------------------
+@torch.enable_grad()        # also inside a backward pass, where autograd is off
+def supervised_loss_grads(flow, gt, mask, scale=20.0):
+    """float64 loss, d loss / d flow, and the elementwise error budget of the float32 kernel's dflow."""
+    from unflow_b200.e2eflow.core import tf_image
+    f32 = 2.0 ** -24
+    H, W = gt.shape[1:3]
+    f = flow.detach().double().requires_grad_(True)
+    v = tf_image.resize_bilinear(f, (H, W)) * scale
+    x = v - gt.double()
+    m = torch.ones_like(x[..., :1]) if mask is None else mask.double()
+    n = float(x.numel())
+    loss = (m * (x * x + EPS2) ** ALPHA).sum() / n
+    dflow, = torch.autograd.grad(loss, f, retain_graph=True)
+    with torch.no_grad():
+        q = x * x + EPS2
+        c = 2 * ALPHA * x * q ** (ALPHA - 1)                         # d/dx of the penalty
+        dc = 2 * ALPHA * q ** (ALPHA - 1) + 4 * ALPHA * (ALPHA - 1) * x * x * q ** (ALPHA - 2)
+        # float32: |x| carries ~8 ulp of |v| + |gt| (the lerps, the scale, the difference); the penalty's
+        # derivative ~1e-5 relative (exp2 / log2 approximations, the gather's fixed-order sum)
+        per_px = m * (1e-5 * c.abs() + dc.abs() * 8 * f32 * (v.abs() + gt.double().abs()))
+    budget, = torch.autograd.grad(v, f, grad_outputs=per_px * scale / n)
+    return loss.detach(), dflow, budget.abs()

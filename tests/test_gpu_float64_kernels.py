@@ -12,7 +12,7 @@ float64 evaluation on absolute values (tests/float64_refs.py), with that file's 
   correlation  the generic kernel (kernel_size 3, stride_1 2, pad != max_displacement, odd H, W % 4 != 0), the
                tiled backward's run-time radius (even r < 10), C not a multiple of the 128-channel slab.
   warps        BORDER_ZERO / BORDER_CLAMP at 4x384x1280x3 and 2-channel flows at 96x320, forward, dflow and the
-               dimage scatter; BORDER_STN forward.
+               dimage scatter; BORDER_CLAMP with a flow a hair below an integer; BORDER_STN forward.
   forward warp forward and backward at 96x320, at a small flow scale and at one where many splats leave.
   Adam         the four entry points at step 1 and 7, with and without the l2 mask.
 
@@ -238,6 +238,34 @@ def test_warp_vs_float64(shape, mode):
     ri, rfl = R.worst_ratio(dimg, di, Ai), R.worst_ratio(dflow, df, Af)
     print("\nout %.3e  dimage %.3e  dflow %.3e" % (rf, ri, rfl))
     assert max(rf, ri, rfl) <= TAU_SUM
+
+
+def test_image_warp_fraction_just_below_an_integer():
+    """image_warp with u = -1.5 * 2^-24 beside a zero tap: the fp32 fraction u - floor(u) = 1 - 1.5 * 2^-24 rounds
+    to 1 - 2^-23, so the left tap weighs 2^-23 instead of 1.5 * 2^-24.  The kernel does what the reference op does;
+    a float64 reference with the exact fraction is off by 1/3 of A here (a stacked network's image_warp in the
+    CSS step reached 4.6e-6 of A that way, over TAU_SUM).  float64_refs takes the fraction from the fp32 rounding."""
+    from unflow_b200 import _native
+    B, H, W, C = 1, 2, 8, 3
+    lib = _native.lib()
+    img = (torch.arange(W, device="cuda") % 2 == 0).float().view(1, 1, W, 1).expand(B, H, W, C).contiguous()
+    flow = torch.zeros(B, H, W, 2, device="cuda")
+    flow[..., 0] = -1.5 * 2.0 ** -24
+    out, grad = torch.empty_like(img), torch.ones_like(img)
+    dflow, dimg = torch.empty_like(flow), torch.zeros_like(img)
+    assert lib.unflow_backward_warp_fwd(img.data_ptr(), flow.data_ptr(), out.data_ptr(), B, H, W, C, 1, _st()) == 0
+    assert lib.unflow_backward_warp_bwd(grad.data_ptr(), img.data_ptr(), flow.data_ptr(), dflow.data_ptr(),
+                                        dimg.data_ptr(), B, H, W, C, 1, _st()) == 0
+    torch.cuda.synchronize()
+    i64, f64 = img.double(), flow.double()
+    ratios = [R.worst_ratio(out, R.warp(i64, f64, 1), R.warp_abs(i64, f64, 1))]
+    di, df, Ai, Af = R.warp_grads(grad.double(), i64, f64, 1)
+    ratios += [R.worst_ratio(dimg, di, Ai), R.worst_ratio(dflow, df, Af)]
+    exact = R.worst_ratio(out[:, :, 1::2], torch.full_like(out[:, :, 1::2], 1.5 * 2.0 ** -24, dtype=torch.float64),
+                          torch.full_like(out[:, :, 1::2], 1.5 * 2.0 ** -24, dtype=torch.float64))
+    print("\nout %.3e  dimage %.3e  dflow %.3e; against the exact fraction %.3e" % (*ratios, exact))
+    assert max(ratios) <= TAU_SUM
+    assert exact > 0.3
 
 
 def test_spatial_transformer_sampler_vs_float64():

@@ -16,8 +16,7 @@ from oracle import flownet as oflownet
 from oracle import supervised as osup
 from unflow_b200 import synthetic as usynth
 import synth
-
-ALPHA, EPS2, F32 = 0.45, 1e-6, 2.0 ** -24
+from float64_refs import supervised_loss_grads
 
 
 def _inputs(B, h, w, H, W, mask_kind, seed):
@@ -33,28 +32,6 @@ def _inputs(B, h, w, H, W, mask_kind, seed):
         mask = (torch.rand(B, H, W, 1, generator=g) < 0.6).float()
         gt = torch.where(mask > 0, gt, torch.full_like(gt, -512.0))
     return flow, gt, mask
-
-
-def _reference64(flow, gt, mask, scale=20.0):
-    """float64 loss, d loss / d flow, and the elementwise error budget of the float32 kernel's dflow."""
-    from unflow_b200.e2eflow.core import tf_image
-    H, W = gt.shape[1:3]
-    f = flow.double().requires_grad_(True)
-    v = tf_image.resize_bilinear(f, (H, W)) * scale
-    x = v - gt.double()
-    m = torch.ones_like(x[..., :1]) if mask is None else mask.double()
-    n = float(x.numel())
-    loss = (m * (x * x + EPS2) ** ALPHA).sum() / n
-    dflow, = torch.autograd.grad(loss, f, retain_graph=True)
-    with torch.no_grad():
-        q = x * x + EPS2
-        c = 2 * ALPHA * x * q ** (ALPHA - 1)                         # d/dx of the penalty
-        dc = 2 * ALPHA * q ** (ALPHA - 1) + 4 * ALPHA * (ALPHA - 1) * x * x * q ** (ALPHA - 2)
-        # float32: |x| carries ~8 ulp of |v| + |gt| (the lerps, the scale, the difference); the penalty's
-        # derivative ~1e-5 relative (exp2 / log2 approximations, the gather's fixed-order sum)
-        per_px = m * (1e-5 * c.abs() + dc.abs() * 8 * F32 * (v.abs() + gt.double().abs()))
-    budget, = torch.autograd.grad(v, f, grad_outputs=per_px * scale / n)
-    return loss.detach(), dflow, budget.abs()
 
 
 def _kernel(flow, gt, mask, grad=1.0, scale=20.0):
@@ -84,7 +61,7 @@ def _kernel(flow, gt, mask, grad=1.0, scale=20.0):
 def test_kernel_vs_float64(shape, mask_kind):
     B, h, w, H, W = shape
     flow, gt, mask = _inputs(B, h, w, H, W, mask_kind, seed=sum(shape) + len(mask_kind))
-    want_loss, want_d, budget = _reference64(flow, gt, mask)
+    want_loss, want_d, budget = supervised_loss_grads(flow, gt, mask)
     got_loss, got_d = _kernel(flow, gt, mask)
     assert torch.isfinite(got_d).all()
     if mask_kind == "zero":

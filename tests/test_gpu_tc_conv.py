@@ -316,13 +316,20 @@ def options(**kv):
             lib.unflow_set_int_option(k.encode(), OPTION_DEFAULTS[k])
 
 
+def real_lib():
+    """The library handle itself, also while a step test's checking proxy stands in for it (the proxy keeps
+    it as `_real`): plan queries made by a check are not calls of the step."""
+    from unflow_b200 import _native
+    lib = _native.lib()
+    return getattr(lib, "_real", lib)
+
+
 def launch_plan(N, Hin, Win, Cin, Hout, Wout, Cout, mode, stride, kh, kw, pad_t, pad_l):
     """What unflow_tc_conv does under the current options (the plan with the two-parity-classes rewrite):
     n_classes, BN, pair_px and the K slices of a launch whose epilogue allows slicing."""
-    from unflow_b200 import _native
     buf = (ctypes.c_int * 1024)()
-    n = _native.lib().unflow_tc_conv_plan(N, Hin, Win, Cin, Hout, Wout, Cout, mode | 4, stride, kh, kw, pad_t, pad_l,
-                                          buf, 1024)
+    n = real_lib().unflow_tc_conv_plan(N, Hin, Win, Cin, Hout, Wout, Cout, mode | 4, stride, kh, kw, pad_t, pad_l,
+                                       buf, 1024)
     assert n > 0, n
     nt = buf[14]
     return {"n_classes": buf[0], "tiles": buf[8] * buf[9] * buf[10], "BN": buf[12], "kblocks": buf[13], "ntaps": nt,

@@ -22,7 +22,7 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-from test_gpu_tc_conv import launch_plan
+from test_gpu_tc_conv import launch_plan, real_lib
 
 pytestmark = pytest.mark.gpu
 
@@ -128,9 +128,8 @@ def _caller(conv_ops):
 def _wgrad_plan(N, Hp, Wp, R, C, stride, kh, kw, pad_t, pad_l):
     """BN, K blocks per work item and work items along K of a tc_wgrad launch (unflow_tc_wgrad_plan)."""
     import ctypes
-    from unflow_b200 import _native
     v = (ctypes.c_int * 15)()
-    assert _native.lib().unflow_tc_wgrad_plan(N, Hp, Wp, R, C, stride, kh, kw, pad_t, pad_l, v) == 15
+    assert real_lib().unflow_tc_wgrad_plan(N, Hp, Wp, R, C, stride, kh, kw, pad_t, pad_l, v) == 15
     return "BN%d kc%d x%d" % (v[11], v[7], v[8])
 
 

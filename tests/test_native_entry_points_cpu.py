@@ -29,6 +29,27 @@ def test_step_checkers_and_pinned_sets_match_the_table():
         assert pinned <= set(EP.STEP_CHECKED) | set(EP.TC_DELEGATED) | set(EP.HOST_ONLY)
 
 
+def _assigned_dict(tree, name):
+    return next(n.value for n in tree.body if isinstance(n, ast.Assign) and isinstance(n.targets[0], ast.Name)
+                and n.targets[0].id == name)
+
+
+def test_variant_checkers_and_pinned_sets_match_the_table():
+    tree = ast.parse(open(os.path.join(HERE, "test_gpu_variant_step_launches.py")).read())
+    checkers = _assigned_dict(tree, "VARIANT_CHECKERS")
+    spread = [v.id for k, v in zip(checkers.keys, checkers.values) if k is None]
+    assert spread == ["CHECKERS"], "VARIANT_CHECKERS must extend the step's CHECKERS"
+    assert {k.value for k in checkers.keys if k is not None} == set(EP.VARIANT_CHECKED)
+    assert not set(EP.VARIANT_CHECKED) & set(EP.STEP_CHECKED)
+    assert set(EP.VARIANT_CHECKED) <= set(EP.STANDALONE)
+    configs = {k.value for k in _assigned_dict(tree, "CONFIGS").keys}
+    assert configs == set(EP.VARIANT_STEP_CALLS) == {"C-chairs", "C-kitti1152", "S-synthia", "cs-cityscapes",
+                                                     "CSS-bench", "CSS-ft-train_all"}
+    checked = set(EP.STEP_CHECKED) | set(EP.VARIANT_CHECKED) | set(EP.TC_DELEGATED) | set(EP.HOST_ONLY)
+    for cid, pinned in EP.VARIANT_STEP_CALLS.items():
+        assert pinned <= checked, "%s calls entry points without a checker: %s" % (cid, sorted(pinned - checked))
+
+
 def test_standalone_entry_points_name_existing_tests():
     for name, ref in EP.STANDALONE.items():
         fname, test = ref.split("::")
