@@ -1,5 +1,5 @@
-// tc_wgrad.cu -- weight gradients of the conv / deconv stacks on the Hopper tensor cores (wgmma, 3xTF32
-// split of BOTH operands in shared memory, fp32 register accumulation, split-K).
+// tc_wgrad.cu -- weight gradients of the conv / deconv stacks on the Hopper tensor cores (wgmma, 3xTF32: P split
+// in registers, G split in shared memory; fp32 register accumulation, split-K).
 //
 // Replaces the library weight-gradient kernels behind tf.gradients of slim.conv2d /
 // slim.conv2d_transpose (reference src/e2eflow/core/flownet.py:166-233, :89-155; train.py:151-152)
@@ -11,10 +11,19 @@
 //   transposed    y = deconv(x, W):   P = x     (rows r = C_in),  G = dL/dy (cols c = C_out), stride 2
 //
 // GEMM view per work item: M = 128 rows of P's channels, N = BN channels of G, K = pixels.  NHWC
-// memory has the channels contiguous and the contraction index (pixels) across rows, while wgmma reads tf32
-// operands K-major only: TMA brings boxes of 32 pixels x 32 channels as they lie in memory, and the split into
-// hi / lo writes them TRANSPOSED (row = channel, 32 pixels per 128-byte row, 128-byte swizzle).  No transposed
-// copy of any activation exists in global memory.
+// memory has the channels contiguous and the contraction index (pixels) across rows.  TMA brings boxes of 32
+// pixels x 32 channels as they lie in memory: P's in the 128-byte swizzle, G's unswizzled.  The A operand (P)
+// comes from registers, so it needs no transpose: each thread loads its tf32 A fragment straight from the raw
+// P box and splits it there.  The B operand (G) is read by wgmma from shared memory, K-major only: the
+// consumers split it into hi / lo planes written TRANSPOSED (row = channel, 32 pixels per 128-byte row,
+// 128-byte swizzle).  No transposed copy of any activation exists in global memory.
+//
+// K order.  A sum over pixels does not depend on their order, and the fragment row of a lane is fixed by the
+// hardware.  With the natural order the 32 lanes of a fragment load hit only 16 banks of the swizzled box, so
+// inside each 8-pixel K step k the K positions 0-3 hold the pixels 8k + 0, 2, 4, 6 and positions 4-7 the pixels
+// 8k + 1, 3, 5, 7: fragment columns t and t + 4 (t = lane % 4) read pixels 8k + 2t and 8k + 2t + 1, and every
+// fragment load is conflict-free.  The G planes are written in the same order
+// (tests/test_tc_wgrad_fragment_model_cpu.py checks both).
 //
 // Work item = (pixel chunk, 128-row block, BN-column block); the BN columns are BN/32 consecutive
 // (tap, 32-channel group) pairs, so a layer with few input channels fills the tile with several taps at
@@ -23,13 +32,16 @@
 // activations are read from HBM once and re-read from L2.
 //   warp 0           TMA into the raw ring: per K block 4 boxes of P (32 px x 32 ch each) and BN/32 boxes of G
 //                    (element stride = the conv stride, tap offset in the start coordinate, zero fill outside)
-//   warpgroups 1, 2  each splits + transposes its 64 rows of P and half of the G tile from a raw slot
-//                    into a split slot and frees the raw slot at once; then (after a barrier over both, since
-//                    both read all of G) issues wgmma m64nBNk8 for its 64 rows:
-//                    lo*hi + hi*lo + hi*hi per 8-pixel K step; every 8 K blocks the wgmma accumulator is
-//                    added to fp32 registers (see tc_conv.cu, "Accuracy"); at the end of the item:
-//                    red.global.add into dW.  A warpgroup whose 64 rows all lie at or past R only splits its
-//                    half of G: no P rows, no wgmma, no epilogue.
+//   warpgroups 1, 2  each splits + transposes half of the G tile from a raw slot into a split slot; then (after
+//                    a barrier over both, since both read all of G), per 8-pixel K step, each thread loads its
+//                    A fragment of P (rows r, r + 8 of the warpgroup's 64) from the raw slot and splits it in
+//                    registers, and the warpgroup issues wgmma m64nBNk8 with A from registers:
+//                    lo*hi + hi*lo + hi*hi, one commit group per K step, two fragment sets alternating (as in
+//                    tc_conv.cu).  A warp frees the raw slot once it has loaded its last fragment from it, and
+//                    the split slot once every MMA group on it has completed.  Every 8 K blocks the wgmma
+//                    accumulator is added to fp32 registers (see tc_conv.cu, "Accuracy"); at the end of the
+//                    item: red.global.add into dW.  A warpgroup whose 64 rows all lie at or past R only splits
+//                    its half of G: no fragments, no wgmma, no epilogue.
 // dW is accumulated with fp32 atomics (split-K partial sums from several CTAs): the caller zeroes
 // it; the order of the additions, hence the last bits, vary from run to run.
 #include "tc_common.cuh"
@@ -57,18 +69,18 @@ struct WgradParams {
   long long pitch_r, pitch_t;       // dW[r * pitch_r + t * pitch_t + c]
 };
 
-// Two rings.  Raw slot (TMA, unswizzled): [P raw] [G raw], per 32-channel group [32 px][32 ch].  Split slot
-// (consumers -> wgmma): [P hi] [P lo] [G hi] [G lo] (K-major, 128-byte swizzle).  A raw slot is free as soon as
-// both warpgroups have split it; a split slot only when the MMAs of both warpgroups on it are done.  Two split
-// slots let split(k + 1) run while MMA(k) reads the other one; the rest of shared memory holds raw slots, so
-// TMA runs several K blocks ahead of the split.  Every part is a multiple of 4 KB.
-//   BN = 128: 2 x 64 KB split + 3 x 32 KB raw;  BN = 64: 2 x 48 KB + 5 x 24 KB;  BN = 32: 2 x 40 KB + 7 x 20 KB
+// Two rings.  Raw slot (TMA): [P raw] [G raw], per 32-channel group [32 px][32 ch]; the P boxes in the 128-byte
+// swizzle (the A fragments are loaded from them), the G boxes unswizzled (the transposing split reads them with
+// conflict-free scalar loads).  Split slot (consumers -> wgmma): [G hi] [G lo] (K-major, 128-byte swizzle).  A raw
+// slot is free once both warpgroups have split its G and loaded their last A fragment from it; a split slot only
+// when the MMAs of both warpgroups on it are done.  Two split slots let split(k + 1) run while MMA(k) reads the
+// other one; the rest of shared memory holds raw slots, so TMA runs several K blocks ahead of the consumers.
+// Every part is a multiple of 4 KB.
+//   BN = 128: 2 x 32 KB split + 5 x 32 KB raw;  BN = 64: 2 x 16 KB + 8 x 24 KB;  BN = 32: 2 x 8 KB + 8 x 20 KB
 template <int BN>
 struct Cfg {
   static constexpr int G_BYTES = BN * KP * 4;
-  static constexpr int A_HI = 0;
-  static constexpr int A_LO = A_HI + A_BYTES;
-  static constexpr int B_HI = A_LO + A_BYTES;
+  static constexpr int B_HI = 0;
   static constexpr int B_LO = B_HI + G_BYTES;
   static constexpr int SPLIT_BYTES = B_LO + G_BYTES;
   static constexpr int SPLIT_STAGES = 2;
@@ -98,16 +110,23 @@ __device__ __forceinline__ int chunk_len(const WgradParams &p, int chunk) {
   return (k0 + p.kc <= p.n_ptiles) ? p.kc : p.n_ptiles - k0;
 }
 
+// Fragment sets of the consumer, as in tc_conv.cu: K step k of a K block uses set k % FRAG_SETS and is one wgmma
+// group; a set is rewritten once wait_group FRAG_SETS - 1 has retired the group that read it, and after the wait
+// of K step FRAG_SETS - 1 only groups of the current K block can still run.
+constexpr int FRAG_SETS = 2;
+static_assert((KP / 8) % FRAG_SETS == 0 && FRAG_SETS <= KP / 8, "fragment sets per K block");
+
 // raw [group][32 px][32 ch] tile -> rows [row0, row0 + rows) of the transposed hi / lo tiles, one float4 of
-// 4 pixels per item; consecutive threads take consecutive rows (conflict-free reads and swizzled writes)
+// 4 K positions per item.  K positions 4c .. 4c + 3 hold the pixels 8 (c / 2) + c % 2 + {0, 2, 4, 6} (the K
+// order of the header).  Consecutive threads take consecutive rows (conflict-free reads and swizzled writes).
 template <int ROWS>
 __device__ __forceinline__ void split_transpose(const float *raw, unsigned char *hi, unsigned char *lo, int row0, int ct) {
 #pragma unroll
   for (int j = 0; j < ROWS * 8 / 128; ++j) {
     const int i = ct + 128 * j;
     const int r = row0 + i % ROWS, c = i / ROWS;
-    const float *src = raw + (r >> 5) * 1024 + (4 * c) * 32 + (r & 31);
-    const float4 v = make_float4(src[0], src[32], src[64], src[96]), h = tf32_hi4(v);
+    const float *src = raw + (r >> 5) * 1024 + (8 * (c >> 1) + (c & 1)) * 32 + (r & 31);
+    const float4 v = make_float4(src[0], src[64], src[128], src[192]), h = tf32_hi4(v);
     const unsigned o = sw128_offset(r, 4 * c);
     *reinterpret_cast<float4 *>(hi + o) = h;
     *reinterpret_cast<float4 *>(lo + o) = sub4(v, h);
@@ -144,6 +163,8 @@ tc_wgrad_kernel(const __grid_constant__ CUtensorMap mapP, const __grid_constant_
   }
   __syncthreads();
 
+  // registers: 40 for warpgroup 0, 232 for the consumers, inside the role branches (see tc_conv.cu)
+  if (warp < 4) setmaxnreg_dec<40>();
   if (warp == 0) {
     // ===================== TMA producer (whole warp converged, one elected lane issues) =====================
     int s = 0;
@@ -186,77 +207,100 @@ tc_wgrad_kernel(const __grid_constant__ CUtensorMap mapP, const __grid_constant_
     }
     if (p.dbg && blockIdx.x == 0 && lane == 0) { p.dbg[0] = t_wait; p.dbg[1] = clock64() - t_all; }
   } else if (warp >= 4) {
-    // ===================== consumers: split + transpose, wgmma, red.add into dW =====================
+    // ===================== consumers: G split, A fragments, wgmma, red.add into dW =====================
+    setmaxnreg_inc<232>();
     const int cw = (warp >> 2) - 1;                  // rows [64 cw, 64 cw + 64) of the 128-row block
     const int ct = threadIdx.x - 128 * (cw + 1);
-    const int row0 = 64 * cw + 16 * (ct >> 5) + (lane >> 2);
+    const int row0 = 64 * cw + 16 * (ct >> 5) + (lane >> 2);     // this thread's accumulator / A rows: row0, row0 + 8
     const int col0 = 2 * (lane & 3);
-    // K blocks consumed so far: K block n uses raw slot n % RAW_STAGES and split slot n % SPLIT_STAGES (one
-    // counter instead of slot and phase registers; the BN = 128 consumer is at the 168-register limit).  The
-    // role timers are 32-bit for the same reason.
+    // K blocks consumed so far: K block n uses raw slot n % RAW_STAGES and split slot n % SPLIT_STAGES
     unsigned n = 0;
-    unsigned t_wait = 0, t_split = 0;
-    const unsigned t_all = (unsigned)clock();
-    // K block n from its raw slot into its split slot: the raw slot is released as soon as this warp has read
-    // it; the split slot is complete (both halves of G, and fenced for wgmma) after the barrier
-    auto split = [&](bool rows) {
+    long long t_wait = 0, t_split = 0, t_all = clock64();   // role timers: blocked on a loaded raw / free split slot
+    // G of K block n from its raw slot into its split slot (this warpgroup's half); the split slot is complete
+    // (both halves, fenced for wgmma) after the barrier.  The raw slot stays in use: the caller frees it.
+    auto split = [&]() {
       const unsigned rs = n % C::RAW_STAGES, rph = (n / C::RAW_STAGES) & 1u;
       const unsigned ss = n % C::SPLIT_STAGES, sph = (n / C::SPLIT_STAGES) & 1u;
-      { const unsigned t0 = (unsigned)clock(); mbar_wait(raw_full(rs), rph); t_wait += (unsigned)clock() - t0; }
-      { const unsigned t0 = (unsigned)clock(); mbar_wait(split_empty(ss), sph ^ 1u); t_split += (unsigned)clock() - t0; }
+      { const long long t0 = clock64(); mbar_wait(raw_full(rs), rph); t_wait += clock64() - t0; }
+      { const long long t0 = clock64(); mbar_wait(split_empty(ss), sph ^ 1u); t_split += clock64() - t0; }
       const float *raw = reinterpret_cast<const float *>(gbase + C::RAW0 + rs * C::RAW_BYTES);
       unsigned char *sp = gbase + ss * C::SPLIT_BYTES;
-      if (rows) split_transpose<64>(raw, sp + C::A_HI, sp + C::A_LO, 64 * cw, ct);
       split_transpose<BN / 2>(raw + C::G_RAW / 4, sp + C::B_HI, sp + C::B_LO, cw * (BN / 2), ct);
-      __syncwarp();
-      if (lane == 0) mbar_arrive(raw_empty(rs));
       fence_proxy_async();
       named_bar_sync(1, 256);                        // both halves of G are split
+      return raw;
     };
     float sum[R], acc[R];
+    unsigned a_hi[FRAG_SETS][4], a_lo[FRAG_SETS][4];
     for (int item = blockIdx.x; item < total_items; item += gridDim.x) {
       const Item w = decode_item(p, item);
       const int iters = chunk_len(p, w.chunk);
       if (w.rb * BM + 64 * cw >= p.R) {
         // all 64 rows of this warpgroup are past R: its half of G only (the other warpgroup reads it)
         for (int it = 0; it < iters; ++it) {
-          split(false);
-          if (lane == 0) mbar_arrive(split_empty(n % C::SPLIT_STAGES));
+          split();
+          __syncwarp();
+          if (lane == 0) {
+            mbar_arrive(raw_empty(n % C::RAW_STAGES));
+            mbar_arrive(split_empty(n % C::SPLIT_STAGES));
+          }
           ++n;
         }
         continue;
       }
 #pragma unroll
       for (int c = 0; c < R; ++c) sum[c] = 0.f;
-      // chunks and their K blocks as in tc_conv.cu: wait_group 1 inside a chunk, acc read only at its end
+      // chunks and their K blocks as in tc_conv.cu: inside a chunk the only waits are wait_group FRAG_SETS - 1
+      // before a fragment set is rewritten; acc is read only at the chunk's end, behind wait_group 0
       for (int c0 = 0; c0 < iters; c0 += p.chunk) {
         const int c1 = c0 + p.chunk < iters ? c0 + p.chunk : iters;
+        int pending = -1;                            // split slot whose MMAs may still be running
         for (int it = c0; it < c1; ++it) {
-          split(true);
-          const unsigned st = base + (n % C::SPLIT_STAGES) * C::SPLIT_BYTES;
-          const unsigned long long a_hi = wgmma_desc_k128(st + C::A_HI + cw * (A_BYTES / 2));
-          const unsigned long long a_lo = wgmma_desc_k128(st + C::A_LO + cw * (A_BYTES / 2));
+          // this thread's A rows row0, row0 + 8 lie in P box row0 / 32, as channels row0 % 32 and row0 % 32 + 8
+          const float *a = split() + (row0 >> 5) * 1024;
+          const int ch = row0 & 31;
+          const unsigned rs = n % C::RAW_STAGES, ss = n % C::SPLIT_STAGES;
+          const unsigned st = base + ss * C::SPLIT_BYTES;
           const unsigned long long b_hi = wgmma_desc_k128(st + C::B_HI), b_lo = wgmma_desc_k128(st + C::B_LO);
-          fence_regs(acc);
-          wgmma_fence();
 #pragma unroll
-          for (int k = 0; k < KP / 8; ++k) {
+          for (int k = 0; k < KP / 8; ++k) {         // K step = 8 pixels = 32 bytes: +2 in 16-byte units
+            unsigned (&hi)[4] = a_hi[k % FRAG_SETS], (&lo)[4] = a_lo[k % FRAG_SETS];
+            wgmma_wait<FRAG_SETS - 1>();             // the group that last read this set has completed
+            fence_regs(acc);
+            if (k == FRAG_SETS - 1) {
+              // every group of the previous K block has completed: free its split slot
+              __syncwarp();
+              if (pending >= 0 && lane == 0) mbar_arrive(split_empty(pending));
+            }
+            // the tf32 A fragment of the K step: a[e] = P[row0 + 8 (e & 1)][pixel 8k + 2 (lane % 4) + (e >> 1)]
+            // (the K order of the header), from the swizzled raw box, split in registers
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {
+              const float x = a[sw128_offset(8 * k + 2 * (lane & 3) + (e >> 1), ch + 8 * (e & 1)) / 4];
+              const float h = tf32_rna_fast(x);
+              hi[e] = __float_as_uint(h);
+              lo[e] = __float_as_uint(x - h);
+            }
+            if (k == KP / 8 - 1) {
+              // the last fragment of this K block is loaded: the raw slot is free as far as this warp goes
+              __syncwarp();
+              if (lane == 0) mbar_arrive(raw_empty(rs));
+            }
+            wgmma_fence();
             const unsigned long long adv = (unsigned long long)(2 * k);
-            Wgmma<BN>::mma(acc, a_lo + adv, b_hi + adv, (it - c0 | k) != 0);
-            Wgmma<BN>::mma(acc, a_hi + adv, b_lo + adv, 1);
-            Wgmma<BN>::mma(acc, a_hi + adv, b_hi + adv, 1);
+            Wgmma<BN>::mma_rs(acc, lo, b_hi + adv, (it - c0 | k) != 0);
+            Wgmma<BN>::mma_rs(acc, hi, b_lo + adv, 1);
+            Wgmma<BN>::mma_rs(acc, hi, b_hi + adv, 1);
+            wgmma_commit();
           }
-          wgmma_commit();
-          wgmma_wait<1>();
-          fence_regs(acc);
-          __syncwarp();
-          if (it > c0 && lane == 0) mbar_arrive(split_empty((n - 1) % C::SPLIT_STAGES));   // MMA(n - 1) done
+          pending = ss;
           ++n;
         }
+        // chunk end: all MMAs have completed; free the last split slot and add the chunk to the fp32 sum
         wgmma_wait<0>();
         fence_regs(acc);
         __syncwarp();
-        if (lane == 0) mbar_arrive(split_empty((n - 1) % C::SPLIT_STAGES));
+        if (lane == 0) mbar_arrive(split_empty(pending));
 #pragma unroll
         for (int c = 0; c < R; ++c) sum[c] += acc[c];
       }
@@ -277,7 +321,7 @@ tc_wgrad_kernel(const __grid_constant__ CUtensorMap mapP, const __grid_constant_
       }
     }
     if (p.dbg && blockIdx.x == 0 && threadIdx.x == 128) {
-      p.dbg[2] = t_wait; p.dbg[3] = (unsigned)clock() - t_all; p.dbg[4] = t_split;
+      p.dbg[2] = t_wait; p.dbg[3] = clock64() - t_all; p.dbg[4] = t_split;
       p.dbg[5] = C::RAW_STAGES; p.dbg[6] = C::SPLIT_STAGES;
     }
   }
@@ -379,7 +423,7 @@ extern "C" int unflow_tc_wgrad(const float *P, int N, int Hp, int Wp, int R, lon
     cuuint64_t strides[3] = {(cuuint64_t)p_pitch * 4, (cuuint64_t)p_pitch * 4 * Wp, (cuuint64_t)p_pitch * 4 * Wp * Hp};
     cuuint32_t box[4] = {32, (cuuint32_t)p.TW, (cuuint32_t)p.TH, (cuuint32_t)p.TN};
     cuuint32_t estr[4] = {1, 1, 1, 1};
-    rc = tc::encode(&mP, P, 4, dims, strides, box, estr, CU_TENSOR_MAP_SWIZZLE_NONE);   // split + transposed by the consumers
+    rc = tc::encode(&mP, P, 4, dims, strides, box, estr);   // 128-byte swizzle: conflict-free A fragment loads
     if (rc) return rc;
   }
   {
@@ -416,7 +460,7 @@ extern "C" int unflow_tc_wgrad_window(const float *P, int N, int Ho, int Wo, int
     cuuint64_t strides[3] = {(cuuint64_t)p_pitch * 4, (cuuint64_t)p_pitch * 4 * Wo, (cuuint64_t)p_pitch * 4 * Wo * Ho};
     cuuint32_t box[4] = {32, (cuuint32_t)p.TW, (cuuint32_t)p.TH, (cuuint32_t)p.TN};
     cuuint32_t estr[4] = {1, 1, 1, 1};
-    rc = tc::encode(&mP, P, 4, dims, strides, box, estr, CU_TENSOR_MAP_SWIZZLE_NONE);   // split + transposed by the consumers
+    rc = tc::encode(&mP, P, 4, dims, strides, box, estr);   // 128-byte swizzle: conflict-free A fragment loads
     if (rc) return rc;
   }
   {
