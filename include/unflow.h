@@ -251,27 +251,13 @@ int unflow_adam_step_dev_l2(float *params, float *grads, float *m, float *v, lon
                             void *stream);
 
 /* ------------------------------------------------------------------------
- * 3xTF32 operand preparation for the conv / deconv stacks (no reference counterpart: the
- * reference runs its slim.conv2d layers in plain fp32 on cuDNN, src/e2eflow/core/flownet.py:174-233).
- * Reads a logical [N,C,H,W] fp32 tensor through arbitrary strides (in floats) and writes the dense
- * NHWC operand of one TF32 library convolution: x = hi + lo (hi = round-to-nearest TF32), three
- * slabs (order 0: hi,hi,lo; order 1: hi,lo,hi) side by side along C (concat_batch = 0, output
- * [N_out, Hp, Wp, 3*C_pad]) or along N (concat_batch = 1, output [3*N_out, Hp, Wp, C_pad]); channels
- * C..C_pad-1, items N..N_out-1 and the spatial border (TF SAME padding, Hp = H+pad_top+pad_bottom)
- * are written as zeros.  C_pad % 4 == 0.
+ * Bias and leaky ReLU of the conv / deconv layers outside the conv kernels (csrc/bias_act.cu;
+ * reference activation flownet.py:84-86).  `act` is the leaky-ReLU OUTPUT of the layer whose
+ * gradient `g` is, and lrelu'(act) = (act > 0 ? 1 : slope).
  * ---------------------------------------------------------------------- */
-int unflow_conv_operand_tf32(const float *x, float *out, int N, int C, int H, int W, long long sN,
-                             long long sC, long long sH, long long sW, int N_out, int C_pad,
-                             int pad_top, int pad_bottom, int pad_left, int pad_right,
-                             int concat_batch, int order, const float *act, float slope,
-                             void *stream);
-/* `act` (optional, dense NHWC [N,H,W,C]): the leaky-ReLU OUTPUT of the layer whose gradient `x`
- * is; the source is multiplied by lrelu'(act) = (act > 0 ? 1 : slope) on the fly (fused
- * leaky_relu backward, reference activation flownet.py:84-86).
- *
- * unflow_bias_lrelu: y = leaky_relu(y + bias[c]) in place on dense NHWC [pixels][C] (C % 4 == 0).
- * unflow_bias_grad_lrelu: gb[c] = sum_pixels g * lrelu'(act)  (act NULL: plain bias gradient);
- * g is read through strides, gb is zeroed by the launcher. */
+/* unflow_bias_lrelu: y = leaky_relu(y + bias[c]) in place on dense NHWC [pixels][C] (C % 4 == 0).
+ * unflow_bias_grad_lrelu: gb[c] = sum_pixels g * lrelu'(act)  (act: dense NHWC [N,H,W,C]; NULL: plain
+ * bias gradient); g is read through strides, gb is zeroed by the launcher. */
 int unflow_bias_lrelu(float *y, const float *bias, long long pixels, int C, float slope, void *stream);
 /* unflow_lrelu_bwd_bias: unflow_bias_grad_lrelu that also writes gpre = g * lrelu'(act) as dense
  * NHWC [N,H,W,C] (NULL: skip) -- the gradient w.r.t. the pre-activation output, the operand of the

@@ -72,7 +72,6 @@ STANDALONE = {
     "unflow_adam_step": "test_gpu_float64_kernels.py::test_adam_entry_points_vs_float64",
     "unflow_adam_step_dev_l2": "test_gpu_float64_kernels.py::test_adam_entry_points_vs_float64",
     "unflow_adam_step_dev": "test_gpu_float64_kernels.py::test_adam_entry_points_vs_float64",
-    "unflow_conv_operand_tf32": "test_gpu_conv3x.py::test_operand_kernel_exact",
     "unflow_supervised_loss_fwd": "test_gpu_supervised.py::test_kernel_vs_float64",
     "unflow_supervised_loss_bwd": "test_gpu_supervised.py::test_kernel_vs_float64",
 }

@@ -1,7 +1,5 @@
-"""Host logic of the tensor-core conv path (core/conv_ops.py) on the CPU: the operand / bias kernels
-are replaced by exact CPU stand-ins (hi = x, lo = 0, so hi*hi' + hi*lo' + lo*hi' = x*w), which leaves
-the concatenation scheme, the padding bookkeeping, the dgrad-as-transposed-conv formulation, the
-fused bias/activation backward and the channel padding to be checked against plain autograd."""
+"""Host logic of the tensor-core conv path (core/conv_ops.py) on the CPU: the space-to-depth form of the
+first layers and the input copy in front of the kernels, against plain float64 autograd."""
 import pytest
 import torch
 import torch.nn.functional as F
@@ -9,85 +7,11 @@ import torch.nn.functional as F
 from unflow_b200.e2eflow.core import conv_ops as co
 
 
-def _lrelu_grad(a):
-    return torch.where(a > 0, torch.ones_like(a), torch.full_like(a, co.LRELU_SLOPE))
-
-
-def _operand_cpu(x, order, concat_batch=False, c_pad=None, n_out=None, pads=(0, 0, 0, 0), act=None):
-    N, C, H, W = x.shape
-    c_pad = co._round4(C) if c_pad is None else c_pad
-    n_out = N if n_out is None else n_out
-    pt, pb, pl, pr = pads
-    if act is not None:
-        x = x * _lrelu_grad(act)
-    xp = F.pad(x, (pl, pr, pt, pb, 0, c_pad - C, 0, n_out - N))
-    z = torch.zeros_like(xp)
-    parts = [xp, xp, z] if order == 0 else [xp, z, xp]       # (hi,hi,lo) / (hi,lo,hi) with lo = 0
-    return torch.cat(parts, 0 if concat_batch else 1)
-
-
-@pytest.fixture
-def cpu_kernels(monkeypatch):
-    monkeypatch.setattr(co, '_operand', _operand_cpu)
-    monkeypatch.setattr(co, '_bias_act_', lambda y, b: F.leaky_relu_(y.add_(b.view(1, -1, 1, 1)), co.LRELU_SLOPE))
-    monkeypatch.setattr(co, '_bias_grad', lambda g, a: (g if a is None else g * _lrelu_grad(a)).sum((0, 2, 3)))
-
-
-@pytest.mark.parametrize("stride,k,pads,cin,cout,act", [(1, 3, (1, 1, 1, 1), 6, 8, False), (2, 5, (1, 2, 1, 2), 6, 8, True),
-                                                        (2, 7, (2, 3, 2, 3), 3, 8, True), (1, 1, (0, 0, 0, 0), 5, 2, False),
-                                                        (2, 3, (0, 1, 0, 1), 7, 12, True),
-                                                        (1, 4, (0, 0, 0, 0), 12, 8, True)])   # the space-to-depth first layer
-def test_conv3x_function_matches_autograd(cpu_kernels, stride, k, pads, cin, cout, act):
-    g = torch.Generator().manual_seed(k * 10 + stride)
-    x = torch.randn(2, cin, 12, 14, dtype=torch.float64, generator=g).requires_grad_(True)
-    w = torch.randn(cout, cin, k, k, dtype=torch.float64, generator=g).requires_grad_(True)
-    b = torch.randn(cout, dtype=torch.float64, generator=g).requires_grad_(True)
-    y = co._Conv3x.apply(x, w, b, stride, pads, act)
-    ref = F.conv2d(F.pad(x, (pads[2], pads[3], pads[0], pads[1])), w, b, stride=stride)
-    if act:
-        ref = F.leaky_relu(ref, co.LRELU_SLOPE)
-    assert y.shape == ref.shape and float((y - ref).abs().max()) < 1e-12
-    go = torch.randn(ref.shape, dtype=torch.float64, generator=g)
-    got = torch.autograd.grad(y, (x, w, b), go)
-    want = torch.autograd.grad(ref, (x, w, b), go)
-    for a_, b_ in zip(got, want):
-        assert a_.shape == b_.shape and float((a_ - b_).abs().max()) < 1e-10
-
-
-@pytest.mark.parametrize("cin,cout,act", [(6, 8, True), (5, 2, False), (8, 4, True)])
-def test_deconv3x_function_matches_autograd(cpu_kernels, cin, cout, act):
-    g = torch.Generator().manual_seed(cin)
-    x = torch.randn(2, cin, 5, 7, dtype=torch.float64, generator=g).requires_grad_(True)
-    w = torch.randn(cin, cout, 4, 4, dtype=torch.float64, generator=g).requires_grad_(True)
-    b = torch.randn(cout, dtype=torch.float64, generator=g).requires_grad_(True)
-    y = co._Deconv3x.apply(x, w, b, act)
-    ref = F.conv_transpose2d(x, w, b, stride=2, padding=1)
-    if act:
-        ref = F.leaky_relu(ref, co.LRELU_SLOPE)
-    assert y.shape == ref.shape and float((y - ref).abs().max()) < 1e-12
-    go = torch.randn(ref.shape, dtype=torch.float64, generator=g)
-    got = torch.autograd.grad(y, (x, w, b), go)
-    want = torch.autograd.grad(ref, (x, w, b), go)
-    for a_, b_ in zip(got, want):
-        assert float((a_ - b_).abs().max()) < 1e-10
-
-
-def test_input_grad_as_transposed_conv_equals_conv2d_input():
-    from torch.nn import grad as nngrad
-    for (H, W, k, s) in [(13, 17, 3, 1), (13, 18, 5, 2), (14, 17, 7, 2), (12, 16, 3, 2), (9, 9, 1, 1), (11, 10, 3, 3)]:
-        Ho, Wo = (H - k) // s + 1, (W - k) // s + 1
-        w = torch.randn(6, 4, k, k, dtype=torch.float64)
-        g = torch.randn(2, 6, Ho, Wo, dtype=torch.float64)
-        want = nngrad.conv2d_input((2, 4, H, W), w, g, stride=s, padding=0)
-        got = co._conv_input_grad((H, W), w, g, s)
-        assert got.shape == want.shape and float((got - want).abs().max()) < 1e-12
-
-
 @pytest.mark.parametrize("C,H,W,k,pads", [(3, 16, 20, 7, (2, 3, 2, 3)), (6, 17, 21, 7, (3, 3, 3, 3)),
                                           (14, 12, 12, 7, (2, 3, 2, 3)), (3, 10, 14, 5, (1, 2, 1, 2))])
-def test_space_to_depth_first_layer_is_the_same_convolution(cpu_kernels, C, H, W, k, pads):
+def test_space_to_depth_operands_are_the_same_convolution(C, H, W, k, pads):
     """7x7 stride-2 conv == 4x4 stride-1 conv over 2x2 pixel blocks (core/conv_ops.py), values and
-    gradients, through the plain conv and through the _Conv3x Function the GPU path uses."""
+    gradients."""
     g = torch.Generator().manual_seed(C + H)
     x = torch.randn(2, C, H, W, dtype=torch.float64, generator=g).requires_grad_(True)
     w = torch.randn(8, C, k, k, dtype=torch.float64, generator=g).requires_grad_(True)
@@ -99,10 +23,31 @@ def test_space_to_depth_first_layer_is_the_same_convolution(cpu_kernels, C, H, W
     assert co._use_space_to_depth(x, w, 2) and not co._use_space_to_depth(xs, ws, 1)
     go = torch.randn(ref.shape, dtype=torch.float64, generator=g)
     want = torch.autograd.grad(ref, (x, w, b), go)
-    for y in (F.leaky_relu(F.conv2d(xs, ws, b), co.LRELU_SLOPE), co._Conv3x.apply(xs, ws, b, 1, (0, 0, 0, 0), True)):
-        assert y.shape == ref.shape and float((y - ref).abs().max()) < 1e-12
-        got = torch.autograd.grad(y, (x, w, b), go, retain_graph=True)
-        for a_, b_ in zip(got, want):
-            assert a_.shape == b_.shape and float((a_ - b_).abs().max()) < 1e-10
+    y = F.leaky_relu(F.conv2d(xs, ws, b), co.LRELU_SLOPE)
+    assert y.shape == ref.shape and float((y - ref).abs().max()) < 1e-12
+    got = torch.autograd.grad(y, (x, w, b), go)
+    for a_, b_ in zip(got, want):
+        assert a_.shape == b_.shape and float((a_ - b_).abs().max()) < 1e-10
     wide = torch.randn(8, 64, 5, 5, dtype=torch.float64)
     assert not co._use_space_to_depth(torch.zeros(1, 64, 8, 8), wide, 2)        # enough channels already
+
+
+@pytest.mark.parametrize("stride,k,H,W,pads", [(2, 3, 21, 27, (1, 1, 1, 1)), (2, 3, 21, 27, (0, 0, 0, 0)),
+                                               (2, 5, 20, 27, (1, 2, 2, 2)), (1, 3, 21, 27, (1, 1, 1, 1))])
+def test_input_copy_leaves_the_convolution_unchanged(stride, k, H, W, pads):
+    """conv_ops._tc_input: a conv over the copy (NHWC, pitch round4(C), a zero row / column appended where H / W
+    is odd at stride 2) with the pads it returns is the conv over the original input, values and dL/dx."""
+    g = torch.Generator().manual_seed(k * 100 + H + W)
+    C = 5
+    x = torch.randn(2, C, H, W, generator=g).requires_grad_(True)     # on the CPU every input is copied
+    w = torch.randn(4, C, k, k, dtype=torch.float64, generator=g)
+    xt, tp = co._tc_input(x, stride, pads)
+    Hc, Wc = (H + H % 2, W + W % 2) if stride == 2 else (H, W)
+    assert xt.shape == (2, C, Hc, Wc) and xt.stride() == (Hc * Wc * 8, 1, Wc * 8, 8)
+    conv = lambda t, p: F.conv2d(F.pad(t.double().contiguous(), (p[2], p[3], p[0], p[1])), w, stride=stride)
+    ref, got = conv(x, pads), conv(xt, tp)
+    assert got.shape == ref.shape and torch.equal(got, ref)
+    go = torch.randn(ref.shape, dtype=torch.float64, generator=g)
+    want, = torch.autograd.grad(ref, x, go)
+    have, = torch.autograd.grad(got, x, go)
+    assert torch.equal(have, want)

@@ -1,5 +1,6 @@
-"""The 3xTF32 tensor-core conv path (core/conv_ops.py + csrc/split.cu): accuracy against float64
-and end-to-end parity of the model against the fp32 oracle at the same tolerances as plain fp32."""
+"""The 3xTF32 tensor-core conv path (core/conv_ops.py): accuracy against float64 and end-to-end parity of
+the model against the fp32 oracle at the same tolerances as plain fp32.  No library convolution runs on a
+CUDA tensor in this mode: the ``mode3x`` fixture makes them raise."""
 import numpy as np
 import pytest
 import torch
@@ -10,11 +11,22 @@ pytestmark = pytest.mark.gpu
 from oracle import flownet as oflownet
 from oracle import unsupervised as ounsup
 import synth
+from test_gpu_step_launches import count_input_copies
+
+
+def _no_library_conv(name, real):
+    def call(*args, **kw):
+        if any(isinstance(a, torch.Tensor) and a.is_cuda for a in args[:2]):
+            raise AssertionError("library convolution %s on a CUDA tensor in 3xtf32 mode" % name)
+        return real(*args, **kw)
+    return call
 
 
 @pytest.fixture
-def mode3x():
+def mode3x(monkeypatch):
     from unflow_b200.e2eflow.core import conv_ops
+    for mod, name in ((F, "conv2d"), (F, "conv_transpose2d"), (torch.nn.grad, "conv2d_weight")):
+        monkeypatch.setattr(mod, name, _no_library_conv(name, getattr(mod, name)))
     old = conv_ops.get_mode()
     conv_ops.set_mode('3xtf32')
     yield
@@ -25,38 +37,40 @@ def rel(a, b):
     return float((a.double() - b).norm() / b.norm())
 
 
-def test_operand_kernel_exact():
-    """csrc/split.cu: exact hi/lo decomposition, channel / batch concatenation, zero padding of
-    channels, items and the TF-SAME border, arbitrary source strides."""
-    from unflow_b200.e2eflow.core.conv_ops import _operand
-    base = torch.randn(3, 7, 9, 6, device="cuda") * 100          # NHWC memory
-    x = base.permute(0, 3, 1, 2)[:, :5]                           # [3,5,7,9] channel-sliced channels_last view
-    s = _operand(x, 0, c_pad=8, pads=(1, 2, 0, 1))               # -> [3, 24, 10, 10]
-    assert s.shape == (3, 24, 10, 10) and s.is_contiguous(memory_format=torch.channels_last)
-    hi, hi2, lo = s[:, 0:8], s[:, 8:16], s[:, 16:24]
-    assert torch.equal(hi, hi2)
-    inner = (slice(None), slice(0, 5), slice(1, 8), slice(0, 9))
-    assert torch.equal((hi + lo)[inner], x)                       # exact decomposition
-    assert int((hi.contiguous().view(torch.int32) & 0x1FFF).abs().max()) == 0   # hi is a TF32 number
-    total = (hi + lo)
-    mask = torch.zeros_like(total, dtype=torch.bool)
-    mask[inner] = True
-    assert float(total[~mask].abs().max()) == 0.0                 # channel pad + spatial border are zeros
-    assert float((lo[inner].abs() / x.abs()).max()) <= 2.0 ** -11
-    # batch concat, order (hi;lo;hi), extra zero items, NCHW-contiguous source (weights)
-    w = torch.randn(5, 3, 4, 4, device="cuda")
-    b = _operand(w, 1, concat_batch=True, c_pad=4, n_out=8)      # -> [24, 4, 4, 4]
-    assert b.shape == (24, 4, 4, 4)
-    h0, l0, h1 = b[0:8], b[8:16], b[16:24]
-    assert torch.equal(h0, h1) and torch.equal((h0 + l0)[:5, :3], w)
-    assert float(h0[5:].abs().max()) == 0.0 and float(h0[:, 3:].abs().max()) == 0.0
+def on_gpu(x, layout):
+    """``x`` (NCHW, CPU) on the GPU: 'nchw' contiguous; 'nhwc' dense NHWC; 'offset' a channel slice of an NHWC
+    buffer starting at channel 1, so its base is 4 bytes past a 16-byte boundary (pitch C + 4); 'pitch' a channel
+    slice of an NHWC buffer of pitch C + 2 (not a multiple of 4 for C % 4 == 0)."""
+    if layout == "nchw":
+        return x.cuda()
+    before, after = {"nhwc": (0, 0), "offset": (1, 3), "pitch": (0, 2)}[layout]
+    N, C, H, W = x.shape
+    buf = torch.zeros(N, H, W, before + C + after)
+    buf[..., before:before + C] = x.permute(0, 2, 3, 1)
+    return buf.cuda()[..., before:before + C].permute(0, 3, 1, 2)
 
 
-@pytest.mark.parametrize("stride,k,pads", [(1, 3, (1, 1, 1, 1)), (2, 5, (1, 2, 1, 2)), (2, 7, (2, 3, 2, 3))])
-def test_conv3x_matches_float64(mode3x, stride, k, pads):
+# (stride, k, pads, H, W, layout).  None of these inputs can be read in place by the tensor-core kernels, so each
+# layer copies its input once (conv_ops._tc_input): NCHW memory, odd extents at stride 2 (the input gradient is a
+# transposed launch and needs even ones; VALID padding shrinks the bottom / right pads below zero), a base that is
+# not 16-byte aligned, a pixel pitch that is not a multiple of 4 floats.
+CONV_CASES = {
+    "1-3-pads0": (1, 3, (1, 1, 1, 1), 20, 28, "nchw"),
+    "2-5-pads1": (2, 5, (1, 2, 1, 2), 20, 28, "nchw"),
+    "2-7-pads2": (2, 7, (2, 3, 2, 3), 20, 28, "nchw"),
+    "odd-2-3": (2, 3, (1, 1, 1, 1), 21, 27, "nhwc"),
+    "odd-2-3-valid": (2, 3, (0, 0, 0, 0), 21, 27, "nhwc"),
+    "unaligned-1-3": (1, 3, (1, 1, 1, 1), 20, 28, "offset"),
+    "pitch-2-3": (2, 3, (0, 1, 0, 1), 20, 28, "pitch"),
+}
+
+
+@pytest.mark.parametrize("case", list(CONV_CASES))
+def test_conv3x_matches_float64(mode3x, monkeypatch, case):
     from unflow_b200.e2eflow.core import conv_ops
+    stride, k, pads, H, W, layout = CONV_CASES[case]
     g = torch.Generator().manual_seed(0)
-    x = torch.randn(2, 24, 20, 28, generator=g)
+    x = torch.randn(2, 24, H, W, generator=g)
     w = torch.randn(16, 24, k, k, generator=g) * 0.1
     b = torch.randn(16, generator=g)
     xd = F.pad(x.double(), (pads[2], pads[3], pads[0], pads[1])).requires_grad_(True)
@@ -64,14 +78,24 @@ def test_conv3x_matches_float64(mode3x, stride, k, pads):
     yd = F.conv2d(xd, wd, bd, stride=stride)
     go = torch.randn(yd.shape, generator=g)
     yd.backward(go.double())
-    xc, wc, bc = x.cuda().requires_grad_(True), w.cuda().requires_grad_(True), b.cuda().requires_grad_(True)
+    xc, wc, bc = on_gpu(x, layout).requires_grad_(True), w.cuda().requires_grad_(True), b.cuda().requires_grad_(True)
+    copies = count_input_copies(monkeypatch, conv_ops)
     y = conv_ops.conv2d(xc, wc, bc, stride, pads)
     y.backward(go.cuda())
-    H, W = x.shape[2], x.shape[3]
+    assert copies == [(2, 24, H, W)]
     gx_ref = xd.grad[:, :, pads[0]:pads[0] + H, pads[2]:pads[2] + W]
     for got, want, name in ((y, yd, "y"), (xc.grad, gx_ref, "dx"), (wc.grad, wd.grad, "dw"), (bc.grad, bd.grad, "db")):
+        assert got.shape == want.shape, name
         e = rel(got.detach().cpu(), want.detach())
         assert e < 3e-5, "%s: rel err %.2e" % (name, e)   # measured: 2e-6 (3x3), 1e-5 (strided 5x5/7x7); 1xTF32 gives ~5e-4
+
+
+@pytest.mark.parametrize("shape,stride", [((16, 24, 3, 5), 1), ((16, 24, 9, 9), 1), ((16, 24, 1, 1), 2)])
+def test_conv3x_rejects_filters_the_kernels_do_not_take(mode3x, shape, stride):
+    from unflow_b200.e2eflow.core import conv_ops
+    x = torch.zeros(2, 24, 20, 28, device="cuda").contiguous(memory_format=torch.channels_last)
+    with pytest.raises(ValueError, match="square k x k filters with stride <= k <= 8"):
+        conv_ops.conv2d(x, torch.zeros(shape, device="cuda"), None, stride, (0, 0, 0, 0))
 
 
 def test_deconv3x_matches_float64(mode3x):
@@ -121,8 +145,8 @@ def test_unsupervised_loss_3xtf32_vs_oracle(mode3x):
 
 @pytest.mark.parametrize("deconv", [False, True])
 def test_fused_bias_leaky_relu_layer_matches_float64(mode3x, deconv):
-    """conv (+bias +leaky ReLU fused in one pass) and its backward (activation derivative folded into
-    the operand kernel, masked bias gradient) against float64."""
+    """conv (+bias +leaky ReLU fused in the kernel's epilogue) and its backward (activation derivative and
+    bias gradient in one pass over the incoming gradient) against float64."""
     from unflow_b200.e2eflow.core import conv_ops
     g = torch.Generator().manual_seed(5)
     x = torch.randn(2, 12, 10, 14, generator=g)
@@ -150,10 +174,11 @@ def test_fused_bias_leaky_relu_layer_matches_float64(mode3x, deconv):
 
 
 @pytest.mark.parametrize("N,C,H,W", [(2, 194, 37, 70), (1, 18, 16, 32), (3, 16, 5, 33), (1, 386, 48, 160)])
-def test_narrow_flow_head_matches_float64(mode3x, N, C, H, W):
+def test_narrow_flow_head_and_input_gradient_match_float64(mode3x, N, C, H, W):
     """csrc/narrow_conv.cu (the 2-channel 3x3 flow heads): forward, weight and bias gradients in
     exact fp32 against float64; ragged tiles, channel-chunk tails, strided incoming gradient,
-    bit-identical repeats (fixed-order reduction)."""
+    bit-identical repeats (fixed-order reduction).  The input gradient runs on the tensor-core kernel at
+    every pixel pitch of the input, including pitches that are not a multiple of 4 (C = 194, 18, 386)."""
     from unflow_b200.e2eflow.core import conv_ops
     gen = torch.Generator().manual_seed(C * 1000 + H)
     x = torch.randn(N, C, H, W, generator=gen)
@@ -191,8 +216,7 @@ def test_narrow_flow_head_matches_float64(mode3x, N, C, H, W):
     # no bias, and the dispatch rule of conv2d
     y3 = conv_ops._NarrowConv3x3.apply(xc.detach(), wc.detach(), None)
     assert rel((y3 + bc.detach().view(1, 2, 1, 1)).cpu(), yd.detach()) < 2e-6
-    tiles = N * ((H + 15) // 16) * ((W + 31) // 32)
-    assert conv_ops._use_narrow(xc, wc, 1, (1, 1, 1, 1)) == (tiles >= conv_ops.NARROW_MIN_TILES)
+    assert conv_ops._use_narrow(xc, wc, 1, (1, 1, 1, 1))
     assert not conv_ops._use_narrow(xc, wc, 2, (1, 1, 1, 1)) and not conv_ops._use_narrow(xc, wc, 1, (0, 1, 0, 1))
 
 

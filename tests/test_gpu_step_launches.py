@@ -423,6 +423,19 @@ class LibProxy:
         return out
 
 
+def count_input_copies(monkeypatch, conv_ops):
+    """Wraps conv_ops._tc_input; the returned list gets the shape of every input the tensor-core layers copy."""
+    real, copies = conv_ops._tc_input, []
+
+    def counted(x, *args):
+        xt, pads = real(x, *args)
+        if xt is not x:
+            copies.append(tuple(x.shape))
+        return xt, pads
+    monkeypatch.setattr(conv_ops, "_tc_input", counted)
+    return copies
+
+
 def run_checked_step(monkeypatch, augment):
     from unflow_b200 import _native
     from unflow_b200 import synthetic as synth
@@ -439,6 +452,7 @@ def run_checked_step(monkeypatch, augment):
         im1, im2 = im1.to(dev), im2.to(dev)
         torch.manual_seed(7)
         proxy = LibProxy(_native.lib())
+        copies = count_input_copies(monkeypatch, conv_ops)
         monkeypatch.setattr(_native, "_lib", proxy)
         try:
             loss = trainer.step(im1, im2)
@@ -447,13 +461,13 @@ def run_checked_step(monkeypatch, augment):
             monkeypatch.setattr(_native, "_lib", proxy._real)
     finally:
         conv_ops.set_mode(prev)
-    return proxy, float(loss)
+    return proxy, copies, float(loss)
 
 
 @pytest.mark.parametrize("augment", [False, True], ids=["plain", "augment"])
 def test_every_other_launch_of_a_training_step(monkeypatch, augment):
     t0 = time.time()
-    proxy, loss = run_checked_step(monkeypatch, augment)
+    proxy, copies, loss = run_checked_step(monkeypatch, augment)
     print("\n" + proxy.table())
     worst = max(proxy.rows, key=lambda r: r[4] / r[5] if r[5] else (0 if r[4] == 0 else float("inf")))
     print("%d checked launches, worst |err|/A by TAU: %s, worst row %s, loss %.6f, %.1f s" % (
@@ -461,6 +475,7 @@ def test_every_other_launch_of_a_training_step(monkeypatch, augment):
         time.time() - t0))
     print("entry points called: %s" % sorted(proxy.calls))
     assert not proxy.unchecked, "entry points without a checker: %s" % sorted(set(proxy.unchecked))
+    assert not copies, "inputs copied for the tensor-core layers: %s" % copies
     bad = [r for r in proxy.rows if not r[4] <= r[5]]
     assert not bad, "over TAU: %s" % bad
     pinned = EP.AUGMENT_STEP_CALLS if augment else EP.PLAIN_STEP_CALLS

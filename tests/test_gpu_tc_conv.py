@@ -247,7 +247,7 @@ def test_conv_ops_layers_run_on_the_tensor_core_kernels():
 @pytest.mark.parametrize("C,hw,act_pitch", [(4, (5, 7), 8), (32, (9, 11), 36), (64, (13, 21), 196), (128, (6, 10), 128),
                                             (200, (7, 9), 204), (2, (5, 6), 4)])
 def test_lrelu_bwd_bias_pass(C, hw, act_pitch):
-    """gpre = g * lrelu'(act) and the bias gradient in one pass (csrc/split.cu), for channel counts that fill
+    """gpre = g * lrelu'(act) and the bias gradient in one pass (csrc/bias_act.cu), for channel counts that fill
     a quarter / half / whole warp of float4 lanes and for the scalar path (C = 2); act is a channel slice
     of a wider NHWC buffer."""
     from unflow_b200.e2eflow.core import conv_ops

@@ -43,7 +43,8 @@ import torch.nn.functional as F
 
 import float64_refs as R
 import native_entry_points as EP
-from test_gpu_step_launches import CHECKERS, TAU_ADAM, TAU_FOLD, TAU_LOSS, TAU_SUM, LibProxy, _corr_args
+from test_gpu_step_launches import (CHECKERS, TAU_ADAM, TAU_FOLD, TAU_LOSS, TAU_SUM, LibProxy, _corr_args,
+                                    count_input_copies)
 from test_gpu_tc_step_launches import TAU, Recorder
 
 pytestmark = pytest.mark.gpu
@@ -159,6 +160,7 @@ def run_checked_step(monkeypatch, params, supervised, B, H, W):
         torch.manual_seed(7)
         proxy = LibProxy(_native.lib(), VARIANT_CHECKERS)
         rec.install(monkeypatch)
+        copies = count_input_copies(monkeypatch, conv_ops)
         monkeypatch.setattr(_native, "_lib", proxy)
         try:
             loss = trainer.step(*batch)
@@ -167,7 +169,7 @@ def run_checked_step(monkeypatch, params, supervised, B, H, W):
             monkeypatch.setattr(_native, "_lib", proxy._real)
     finally:
         conv_ops.set_mode(prev)
-    return proxy, rec, trainer, float(loss)
+    return proxy, rec, copies, trainer, float(loss)
 
 
 def worst_by_family(proxy, rec):
@@ -231,7 +233,7 @@ def path_misses(cid, proxy, rec, trainer):
 @pytest.mark.parametrize("cid", list(CONFIGS))
 def test_every_launch_of_a_variant_step(monkeypatch, cid):
     t0 = time.time()
-    proxy, rec, trainer, loss = run_checked_step(monkeypatch, *CONFIGS[cid])
+    proxy, rec, copies, trainer, loss = run_checked_step(monkeypatch, *CONFIGS[cid])
     print("\n" + proxy.table())
     print(rec.table())
     print("%s: %d + %d checked launches, worst |err|/A by family: %s, loss %.6f, %.1f s" % (
@@ -239,6 +241,7 @@ def test_every_launch_of_a_variant_step(monkeypatch, cid):
         time.time() - t0))
     print("entry points called: %s" % sorted(proxy.calls))
     assert not proxy.unchecked, "entry points without a checker: %s" % sorted(set(proxy.unchecked))
+    assert not copies, "inputs copied for the tensor-core layers: %s" % copies
     bad = [r for r in proxy.rows if not r[4] <= r[5]]
     assert not bad, "over TAU: %s" % bad
     bad_tc = [i for i, r in enumerate(rec.rows) if not r["ratio"] <= TAU]

@@ -57,5 +57,5 @@ def test_standalone_entry_points_name_existing_tests():
         funcs = {n.name for n in tree.body if isinstance(n, ast.FunctionDef)}
         assert test in funcs, "%s: %s does not exist" % (name, ref)
         body = open(os.path.join(HERE, fname)).read()
-        assert name[len("unflow_"):] in body or name in body or fname == "test_gpu_supervised.py" \
-            or fname == "test_gpu_conv3x.py", "%s is not exercised in %s" % (name, fname)
+        assert name[len("unflow_"):] in body or name in body or fname == "test_gpu_supervised.py", \
+            "%s is not exercised in %s" % (name, fname)

@@ -14,7 +14,7 @@ sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 from unflow_b200 import synthetic as synth  # noqa: E402
 from unflow_b200.e2eflow import ops  # noqa: E402
-from unflow_b200.e2eflow.core import fused_loss, conv_ops  # noqa: E402
+from unflow_b200.e2eflow.core import fused_loss  # noqa: E402
 from unflow_b200.e2eflow.core.image_warp import image_warp  # noqa: E402
 from unflow_b200 import _native  # noqa: E402
 
@@ -50,11 +50,6 @@ def main():
         _native.check(_native.lib().unflow_adam_step(p.data_ptr(), g.data_ptr(), m.data_ptr(), v.data_ptr(), n,
                                                      1e-4, 0.9, 0.999, 1e-8, t, 1.0, 1,
                                                      torch.cuda.current_stream().cuda_stream), "adam")
-    # the conv-operand kernel on the input of conv3_1 (conv_redir + both correlation volumes)
-    conv_ops.set_mode('3xtf32')
-    x = torch.randn(8, 48, 160, 473, device="cuda").permute(0, 3, 1, 2)
-    for _ in range(reps):
-        conv_ops._operand(x, 0, pads=(1, 1, 1, 1))
     torch.cuda.synchronize()
 
 

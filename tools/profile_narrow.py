@@ -1,8 +1,8 @@
 #!/usr/bin/env python
-"""The narrow-conv kernels (flow heads) and the conv-operand kernel at the shapes of the benchmark
-step, one launch each, for `ncu --set full`:
+"""The narrow-conv kernels (flow heads) at the shapes of the benchmark step, one launch each, for
+`ncu --set full`:
 
-  ncu --set full --clock-control none --import-source on -k regex:"narrow_|conv_operand" \
+  ncu --set full --clock-control none --import-source on -k regex:"narrow_" \
       -o gpurun_out/prof_narrow python tools/profile_narrow.py
 """
 import os

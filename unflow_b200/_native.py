@@ -47,8 +47,6 @@ SIGNATURES = {
     "unflow_forward_warp_fwd": (_i, [_vp] * 2 + [_i] * 3 + [_vp]),
     "unflow_forward_warp_bwd": (_i, [_vp] * 3 + [_i] * 3 + [_vp]),
     "unflow_downsample": (_i, [_vp] * 2 + [_i] * 5 + [_vp]),
-    "unflow_conv_operand_tf32": (_i, [_vp, _vp] + [_i] * 4 + [ctypes.c_longlong] * 4 + [_i] * 8 +
-                                 [_vp, ctypes.c_float, _vp]),
     "unflow_bias_lrelu": (_i, [_vp, _vp, ctypes.c_longlong, _i, ctypes.c_float, _vp]),
     "unflow_bias_grad_lrelu": (_i, [_vp] + [ctypes.c_longlong] * 4 + [_vp, _vp] + [_i] * 4 +
                                [ctypes.c_float, _vp]),

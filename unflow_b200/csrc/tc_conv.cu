@@ -427,7 +427,7 @@ int set_tc_pair_px(int v) { if (v != 0 && v != 1) return 0; tc::g_pair_px = v; r
 
 using namespace unflow;
 
-extern "C" int unflow_bias_lrelu(float *y, const float *bias, long long pixels, int C, float slope, void *stream);   // split.cu
+extern "C" int unflow_bias_lrelu(float *y, const float *bias, long long pixels, int C, float slope, void *stream);   // bias_act.cu
 
 extern "C" int unflow_tc_wsplit(const float *w, float *w_hi, float *w_lo, int taps, int R, int C, long long s_t,
                                 long long s_r, long long s_c, void *stream) {

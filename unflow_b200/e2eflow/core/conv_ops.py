@@ -1,4 +1,4 @@
-"""conv / deconv layers of the FlowNet stacks with a selectable arithmetic mode.
+"""conv / deconv layers of the FlowNet stacks in one of two arithmetic modes.
 
 'fp32'    plain cuDNN float32 (what the reference's slim.conv2d computes, flownet.py:174-233);
           no tensor cores.
@@ -8,13 +8,11 @@
           and input gradient, csrc/tc_wgrad.cu: weight gradient, csrc/narrow_conv*.cu: the 2-channel flow
           heads in exact fp32) with the K loop cut into chunks that are summed in fp32 registers: 1.8e-6 of
           max|y| against float64 per layer, and the same 1e-4 flow tolerance against the fp32 oracle as the
-          plain fp32 path.  Layers these kernels do not serve (tensors that are not NHWC / 16-byte aligned) fall
-          back to cuDNN TF32 convolutions fed the split operands (csrc/split.cu, the round-1 path).
-'tf32'    single-pass TF32 (reduced precision; never used for parity or the headline number).
+          plain fp32 path.  Every layer runs on these kernels; an input they cannot read in place is copied
+          into a fresh NHWC buffer first (_tc_input).
 """
 import torch
 import torch.nn.functional as F
-from torch.nn import grad as nngrad
 
 from ... import _native
 from ..._native import check
@@ -24,8 +22,8 @@ _MODE = 'fp32'
 
 def set_mode(mode):
     global _MODE
-    if mode not in ('fp32', '3xtf32', 'tf32'):
-        raise ValueError("conv precision must be 'fp32', '3xtf32' or 'tf32'")
+    if mode not in ('fp32', '3xtf32'):
+        raise ValueError("conv precision must be 'fp32' or '3xtf32'")
     _MODE = mode
     # the flag is process-global because autograd runs the backward convolutions later
     torch.backends.cudnn.allow_tf32 = mode != 'fp32'
@@ -59,7 +57,6 @@ _backward_point_cb = None
 # ---------------------------------------------------------------------------------------------
 _generation = 0
 _grad_slots = {}
-_GRAD_SLOTS = __import__('os').environ.get('UNFLOW_GRAD_SLOTS', '1') != '0'
 
 
 def new_forward_generation():
@@ -76,13 +73,12 @@ def _slot_key(x):
 
 
 def grad_slot_get(gen, x, key=None):
-    return _grad_slots.get(gen, {}).get(key if key is not None else _slot_key(x)) if _GRAD_SLOTS else None
+    return _grad_slots.get(gen, {}).get(key if key is not None else _slot_key(x))
 
 
 def grad_slot_put(gen, key_or_tensor, g):
-    if _GRAD_SLOTS:
-        key = key_or_tensor if isinstance(key_or_tensor, tuple) else _slot_key(key_or_tensor)
-        _grad_slots.setdefault(gen, {})[key] = g
+    key = key_or_tensor if isinstance(key_or_tensor, tuple) else _slot_key(key_or_tensor)
+    _grad_slots.setdefault(gen, {})[key] = g
 
 
 def set_backward_point_callback(fn):
@@ -112,16 +108,6 @@ def backward_point(x, name):
     return _BackwardPoint.apply(x, name)
 
 
-def _bias_act_(y, b):
-    """y = leaky_relu(y + b) in place (one pass instead of bias add + activation)."""
-    N, C, H, W = y.shape
-    assert y.is_contiguous(memory_format=torch.channels_last) and C % 4 == 0
-    with torch.cuda.device(y.device):
-        check(_native.lib().unflow_bias_lrelu(y.data_ptr(), b.data_ptr(), N * H * W, C, LRELU_SLOPE,
-                                              torch.cuda.current_stream().cuda_stream), "bias_lrelu")
-    return y
-
-
 def _bias_grad(g, act):
     """sum over pixels of g * lrelu'(act) (act None: plain sum) -> [C]."""
     N, C, H, W = g.shape
@@ -139,165 +125,10 @@ def _round4(c):
     return (c + 3) // 4 * 4
 
 
-def _operand(x, order, concat_batch=False, c_pad=None, n_out=None, pads=(0, 0, 0, 0), act=None):
-    """One pass of csrc/split.cu: logical [N,C,H,W] (any strides) -> the dense channels_last TF32
-    operand [N_out, 3*C_pad, Hp, Wp] (channel concat) or [3*N_out, C_pad, Hp, Wp] (batch concat)."""
-    N, C, H, W = x.shape
-    c_pad = _round4(C) if c_pad is None else c_pad
-    n_out = N if n_out is None else n_out
-    pt, pb, pl, pr = pads
-    Hp, Wp = H + pt + pb, W + pl + pr
-    out = torch.empty((3 * n_out * Hp * Wp * c_pad,), device=x.device, dtype=torch.float32)
-    sN, sC, sH, sW = x.stride()
-    from ..ops import kernel_timer
-    with torch.cuda.device(x.device), kernel_timer.span("conv_operand", 4 * x.numel() + 4 * out.numel()):
-        check(_native.lib().unflow_conv_operand_tf32(
-            x.data_ptr(), out.data_ptr(), N, C, H, W, sN, sC, sH, sW, n_out, c_pad, pt, pb, pl, pr,
-            1 if concat_batch else 0, order, act.data_ptr() if act is not None else None, LRELU_SLOPE,
-            torch.cuda.current_stream().cuda_stream), "conv_operand_tf32")
-    if concat_batch:
-        return out.view(3 * n_out, Hp, Wp, c_pad).permute(0, 3, 1, 2)
-    return out.view(n_out, Hp, Wp, 3 * c_pad).permute(0, 3, 1, 2)
-
-
-def _conv_input_grad(input_hw, weight, grad_output, stride):
-    """Gradient of ``conv2d(x, weight, stride=stride, padding=0)`` w.r.t. ``x`` ([.., input_hw]).
-
-    Written as the transposed convolution it is (output_padding recovers the rows / columns a
-    strided conv leaves unused).  ``torch.nn.grad.conv2d_input`` computes the same thing but hands
-    cuDNN a stride-0 placeholder for ``x``; ATen then aligns ``grad_output`` to THAT tensor's
-    (NCHW) format and back to the weight's NHWC -- two full copies of the 3x-wide gradient operand
-    per layer."""
-    sh, sw = (stride, stride) if isinstance(stride, int) else stride
-    kh, kw = weight.shape[2], weight.shape[3]
-    oph = input_hw[0] - ((grad_output.shape[2] - 1) * sh + kh)
-    opw = input_hw[1] - ((grad_output.shape[3] - 1) * sw + kw)
-    assert 0 <= oph < max(sh, 1) and 0 <= opw < max(sw, 1), (input_hw, grad_output.shape, stride)
-    return F.conv_transpose2d(grad_output, weight, None, stride=(sh, sw), padding=0,
-                              output_padding=(oph, opw))
-
-
-def _pad_bias(b, co_p):
-    if b is None or b.shape[0] == co_p:
-        return b
-    return F.pad(b, (0, co_p - b.shape[0]))
-
-
-class _Conv3x(torch.autograd.Function):
-    """conv2d(pad_same(x), w) + b at fp32-level accuracy on the tensor cores (one TF32 cuDNN conv
-    over the channel-concatenated hi/lo operands).  ``pads`` = TF SAME (top, bottom, left, right)."""
-
-    @staticmethod
-    def forward(ctx, x, w, b, stride, pads, act):
-        Co, Ci = w.shape[0], w.shape[1]
-        ci_p, co_p = _round4(Ci), _round4(Co)
-        fuse = bool(act) and b is not None and co_p == Co
-        xs = _operand(x, 0, c_pad=ci_p, pads=pads)               # [N, 3Ci_p, Hp, Wp]  hi,hi,lo
-        ws = _operand(w, 1, c_pad=ci_p, n_out=co_p)              # [Co_p, 3Ci_p, k, k] hi,lo,hi
-        if fuse:     # conv -> (bias + leaky ReLU) in one in-place pass
-            y = _bias_act_(F.conv2d(xs, ws, None, stride=stride, padding=0), b)
-            ctx.save_for_backward(x, w, y)
-        else:
-            assert not act, "fused activation needs a bias and C_out % 4 == 0"
-            y = F.conv2d(xs, ws, _pad_bias(b, co_p), stride=stride, padding=0)
-            ctx.save_for_backward(x, w)
-        ctx.cfg = (stride, pads, b is not None, ci_p, co_p)
-        ctx.fuse = fuse
-        return y if co_p == Co else y[:, :Co]
-
-    @staticmethod
-    def backward(ctx, g):
-        if ctx.fuse:
-            x, w, a = ctx.saved_tensors
-        else:
-            (x, w), a = ctx.saved_tensors, None
-        stride, pads, has_b, ci_p, co_p = ctx.cfg
-        Co, Ci, k = w.shape[0], w.shape[1], w.shape[2]
-        N, _, H, W = x.shape
-        pt, pb, pl, pr = pads
-        gx = gw = gb = None
-
-        def input_grad():
-            gs = _operand(g, 0, c_pad=co_p, act=a)                                 # [N, 3Co_p, ..]
-            wt = _operand(w, 1, concat_batch=True, c_pad=ci_p, n_out=co_p)        # [3Co_p, Ci_p, k, k]
-            gxp = _conv_input_grad((H + pt + pb, W + pl + pr), wt, gs, stride)
-            return gxp[:, :Ci, pt:pt + H, pl:pl + W]
-
-        def weight_grad():
-            xb = _operand(x, 0, concat_batch=True, c_pad=ci_p, pads=pads)          # [3N, Ci_p, Hp, Wp]
-            gb3 = _operand(g, 1, concat_batch=True, c_pad=co_p, act=a)             # [3N, Co_p, ..]
-            gwp = nngrad.conv2d_weight(xb, (co_p, ci_p, k, k), gb3, stride=stride, padding=0)
-            return gwp[:Co, :Ci], (gwp,)
-
-        if ctx.needs_input_grad[0]:
-            gx = input_grad()
-        if ctx.needs_input_grad[1]:
-            gw = weight_grad()[0]
-        if has_b and ctx.needs_input_grad[2]:
-            gb = _bias_grad(g, a)
-        return gx, gw, gb, None, None, None
-
-
-class _Deconv3x(torch.autograd.Function):
-    """conv_transpose2d(x, w[in,out,4,4], stride=2, padding=1) + b, same scheme."""
-
-    @staticmethod
-    def forward(ctx, x, w, b, act):
-        Ci, Co = w.shape[0], w.shape[1]
-        ci_p, co_p = _round4(Ci), _round4(Co)
-        fuse = bool(act) and b is not None and co_p == Co
-        xs = _operand(x, 0, c_pad=ci_p)                                           # [N, 3Ci_p, h, w]
-        ws = _operand(w, 1, concat_batch=True, c_pad=co_p, n_out=ci_p)            # [3Ci_p, Co_p, 4, 4]
-        if fuse:
-            y = _bias_act_(F.conv_transpose2d(xs, ws, None, stride=2, padding=1), b)
-            ctx.save_for_backward(x, w, y)
-        else:
-            assert not act, "fused activation needs a bias and C_out % 4 == 0"
-            y = F.conv_transpose2d(xs, ws, _pad_bias(b, co_p), stride=2, padding=1)
-            ctx.save_for_backward(x, w)
-        ctx.cfg = (b is not None, ci_p, co_p)
-        ctx.fuse = fuse
-        return y if co_p == Co else y[:, :Co]
-
-    @staticmethod
-    def backward(ctx, g):
-        if ctx.fuse:
-            x, w, a = ctx.saved_tensors
-        else:
-            (x, w), a = ctx.saved_tensors, None
-        has_b, ci_p, co_p = ctx.cfg
-        Ci, Co = w.shape[0], w.shape[1]
-        gx = gw = gb = None
-
-        def input_grad():
-            gs = _operand(g, 0, c_pad=co_p, act=a)                                # [N, 3Co_p, 2h, 2w]
-            wc = _operand(w, 1, c_pad=co_p, n_out=ci_p)                           # [Ci_p, 3Co_p, 4, 4]
-            gxp = F.conv2d(gs, wc, None, stride=2, padding=1)
-            return gxp if ci_p == Ci else gxp[:, :Ci]
-
-        def weight_grad():
-            # d/dw of conv_transpose == weight gradient of the conv whose input is g and output x
-            gb3 = _operand(g, 0, concat_batch=True, c_pad=co_p, act=a)
-            xb = _operand(x, 1, concat_batch=True, c_pad=ci_p)
-            gwp = nngrad.conv2d_weight(gb3, (ci_p, co_p, 4, 4), xb, stride=2, padding=1)
-            return gwp[:Ci, :Co], (gwp,)
-
-        if ctx.needs_input_grad[0]:
-            gx = input_grad()
-        if ctx.needs_input_grad[1]:
-            gw = weight_grad()[0]
-        if has_b and ctx.needs_input_grad[2]:
-            gb = _bias_grad(g, a)
-        return gx, gw, gb, None
-
-
 # ---------------------------------------------------------------------------------------------
-# Hand-written tensor-core path (csrc/tc_conv.cu): wgmma implicit GEMM, 3xTF32 split in shared
-# memory, fused bias / leaky ReLU.  Forward and input gradient; the weight gradient still goes
-# through the library path below (round-2 work in progress: csrc/tc_wgrad).
+# Hand-written tensor-core path (3xTF32 wgmma implicit GEMM): csrc/tc_conv.cu for the forward (fused
+# bias / leaky ReLU) and the input gradient, csrc/tc_wgrad.cu for the weight gradient.
 # ---------------------------------------------------------------------------------------------
-_TC = __import__('os').environ.get('UNFLOW_TC_CONV', '1') != '0'
-_TC_WGRAD = __import__('os').environ.get('UNFLOW_TC_WGRAD', '1') != '0'
 
 
 def _grad_slot(w):
@@ -327,10 +158,30 @@ def _tc_weight_grad(P, G, w, stride, pad_t, pad_l):
     return tc_conv.wgrad(P, G, gw, stride=stride, kh=kh, kw=kw, pad_t=pad_t, pad_l=pad_l)
 
 
-def _tc_ok(x, stride):
+def _tc_input(x, stride=1, pads=(0, 0, 0, 0)):
+    """``x`` and its ``pads`` (top, bottom, left, right) as _ConvTC / _DeconvTC take them.
+
+    The kernels read NHWC memory with a 16-byte aligned base and a pixel pitch that is a multiple of 4
+    floats, and the input gradient of a stride-2 conv (a transposed launch) needs an even H and W.  Any other
+    input is copied into a fresh NHWC buffer of pitch round4(C), one zero row / column longer at the bottom /
+    right where H / W is odd at stride 2.  The copy is differentiable: autograd returns dL/dx through it.
+    The bottom / right pads shrink by what was appended, so the output extent is that of ``x``; the kernels
+    read the appended zeros as they read their own TMA zero fill, so the result is the same.  No FlowNet
+    layer takes the copy: the network inputs and the concat buffers are already in this form."""
     from . import tc_conv
-    return (_TC and _MODE == '3xtf32' and x.is_cuda and tc_conv.supported(x)
-            and (stride == 1 or (x.shape[2] % 2 == 0 and x.shape[3] % 2 == 0)))
+    N, C, H, W = x.shape
+    eh, ew = (H % 2, W % 2) if stride == 2 else (0, 0)
+    if tc_conv.supported(x) and not (eh or ew):
+        return x, pads
+    buf = torch.zeros((N, H + eh, W + ew, _round4(C)), device=x.device, dtype=torch.float32)
+    buf[:, :H, :W, :C] = x.permute(0, 2, 3, 1)
+    xt = buf[..., :C].permute(0, 3, 1, 2)
+    # The copy is new memory, so no gradient slot can belong to it.  One keyed by its address is left by an
+    # earlier, freed tensor of this forward generation (layers called one after another outside a network
+    # forward pass, which would start a new generation): drop it, or the backward would add dL/dx into it.
+    _grad_slots.get(_generation, {}).pop(_slot_key(xt), None)
+    pt, pb, pl, pr = pads
+    return xt, (pt, pb - eh, pl, pr - ew)
 
 
 def _khwc(w):
@@ -429,9 +280,8 @@ class _ConvTC(torch.autograd.Function):
         from . import tc_conv
         x, w, a = ctx.saved_tensors
         stride, pads, has_b, act = ctx.cfg
-        Co, Ci, k = w.shape[0], w.shape[1], w.shape[2]
-        N, _, H, W = x.shape
-        pt, pb, pl, pr = pads
+        k = w.shape[2]
+        pt, _, pl, _ = pads
         gx = gw = gb = None
         gpre, gb_all = _lrelu_bwd_bias(g, a if act else None, has_b and ctx.needs_input_grad[2])
         if has_b and ctx.needs_input_grad[2]:
@@ -442,13 +292,7 @@ class _ConvTC(torch.autograd.Function):
                 gpre, tc_conv.split_weights(_khwc(w), transpose=True), dst, mode=1,
                 stride=stride, kh=k, kw=k, pad_t=pt, pad_l=pl, accumulate=acc))
         if ctx.needs_input_grad[1]:
-            if _TC_WGRAD and tc_conv.supported(gpre):
-                gw = _tc_weight_grad(gpre, x, w, stride, pt, pl)                   # rows C_out, columns C_in
-            else:
-                ci_p, co_p = _round4(Ci), _round4(Co)
-                xb = _operand(x, 0, concat_batch=True, c_pad=ci_p, pads=pads)      # [3N, Ci_p, Hp, Wp]
-                gb3 = _operand(gpre, 1, concat_batch=True, c_pad=co_p)             # [3N, Co_p, ..]
-                gw = nngrad.conv2d_weight(xb, (co_p, ci_p, k, k), gb3, stride=stride, padding=0)[:Co, :Ci]
+            gw = _tc_weight_grad(gpre, x, w, stride, pt, pl)                       # rows C_out, columns C_in
         return gx, gw, gb, None, None, None, None
 
 
@@ -492,13 +336,9 @@ class _ConvWindow(torch.autograd.Function):
         return None, gw, gb, None, None, None, None
 
 
-_WINDOW = __import__('os').environ.get('UNFLOW_CONV1_WINDOW', '1') != '0'
-
-
 def _use_window(x, w, stride):
-    return (_WINDOW and _TC and _TC_WGRAD and _MODE == '3xtf32' and x.is_cuda and stride in (2, (2, 2))
-            and w.shape[2] == w.shape[3] and 5 <= w.shape[2] <= 8 and w.shape[1] <= 16 and w.shape[0] % 4 == 0
-            and not x.requires_grad)
+    return (stride in (2, (2, 2)) and w.shape[2] == w.shape[3] and 5 <= w.shape[2] <= 8 and w.shape[1] <= 16
+            and w.shape[0] % 4 == 0 and not x.requires_grad)
 
 
 class _DeconvTC(torch.autograd.Function):
@@ -522,8 +362,6 @@ class _DeconvTC(torch.autograd.Function):
         from . import tc_conv
         x, w, a = ctx.saved_tensors
         has_b, act = ctx.cfg
-        Ci, Co = w.shape[0], w.shape[1]
-        N, _, H, W = x.shape
         gx = gw = gb = None
         gpre, gb_all = _lrelu_bwd_bias(g, a if act else None, has_b and ctx.needs_input_grad[2])
         if has_b and ctx.needs_input_grad[2]:
@@ -534,13 +372,7 @@ class _DeconvTC(torch.autograd.Function):
                 gpre, tc_conv.split_weights(_khwc(w)), dst, mode=0, stride=2, kh=4,
                 kw=4, pad_t=1, pad_l=1, accumulate=acc))
         if ctx.needs_input_grad[1]:
-            if _TC_WGRAD and tc_conv.supported(gpre):
-                gw = _tc_weight_grad(x, gpre, w, 2, 1, 1)                          # rows C_in, columns C_out
-            else:
-                ci_p, co_p = _round4(Ci), _round4(Co)
-                gb3 = _operand(gpre, 0, concat_batch=True, c_pad=co_p)
-                xb = _operand(x, 1, concat_batch=True, c_pad=ci_p)
-                gw = nngrad.conv2d_weight(gb3, (ci_p, co_p, 4, 4), xb, stride=2, padding=1)[:Ci, :Co]
+            gw = _tc_weight_grad(x, gpre, w, 2, 1, 1)                              # rows C_in, columns C_out
         return gx, gw, gb, None, None
 
 
@@ -548,38 +380,21 @@ class _DeconvTC(torch.autograd.Function):
 # fill the GPU with 16x32-pixel tiles, the coarse ones (flow4 .. flow6: 8 .. 48 tiles) split the input
 # channels over several CTAs per tile (csrc/narrow_conv.cu, csplit).  On the tensor-core kernel a head is
 # one 32-wide N block with 2 useful columns and a K of 9 x 1026 walked by a handful of CTAs: 0.5 ms per step.
-NARROW_MIN_TILES = 1
-_NARROW = __import__('os').environ.get('UNFLOW_NARROW_CONV', '1') != '0'
-
-
-def _narrow_lib():
-    return _native.lib()
-
-
-def _narrow_tiles(N, H, W):
-    return N * ((H + 15) // 16) * ((W + 31) // 32)
-
-
 def _use_narrow(x, w, stride, pads):
     from . import tc_conv
-    return (_NARROW and w.shape[0] == 2 and w.shape[2] == 3 and w.shape[3] == 3 and stride in (1, (1, 1))
+    return (w.shape[0] == 2 and w.shape[2] == 3 and w.shape[3] == 3 and stride in (1, (1, 1))
             and tuple(pads) == (1, 1, 1, 1) and x.shape[1] % 2 == 0 and x.dtype == torch.float32
-            and tc_conv.nhwc_geometry(x) is not None        # NHWC memory, possibly a slice of a concat buffer
-            and _narrow_tiles(x.shape[0], x.shape[2], x.shape[3]) >= NARROW_MIN_TILES)
-
-
-def _pixel_pitch(x):
-    from . import tc_conv
-    return tc_conv.nhwc_geometry(x)[4]
+            and tc_conv.nhwc_geometry(x) is not None)       # NHWC memory, possibly a slice of a concat buffer
 
 
 class _NarrowConv3x3(torch.autograd.Function):
     """The 2-channel flow heads (csrc/narrow_conv.cu): forward and weight gradient in exact fp32 on
-    the FMA pipes, reading the wide input once; the input gradient (C_in wide) keeps the
-    tensor-core path of ``_Conv3x``."""
+    the FMA pipes, reading the wide input once at any pixel pitch; the input gradient (C_in wide) runs
+    on the tensor-core kernel."""
 
     @staticmethod
     def forward(ctx, x, w, b):
+        from . import tc_conv
         N, C, H, W = x.shape
         wl = w if w.is_contiguous(memory_format=torch.channels_last) else \
             w.contiguous(memory_format=torch.channels_last)
@@ -587,9 +402,9 @@ class _NarrowConv3x3(torch.autograd.Function):
         y = torch.empty((N, H, W, 4), device=x.device, dtype=torch.float32)[..., :2].permute(0, 3, 1, 2)
         from ..ops import kernel_timer
         with torch.cuda.device(x.device), kernel_timer.span("narrow_conv_fwd", 4 * x.numel() + 4 * y.numel()):
-            check(_narrow_lib().unflow_conv3x3_narrow_fwd(
-                x.data_ptr(), _pixel_pitch(x), wl.data_ptr(), b.data_ptr() if b is not None else None, y.data_ptr(),
-                4, N, H, W, C, 2, torch.cuda.current_stream().cuda_stream), "conv3x3_narrow_fwd")
+            check(_native.lib().unflow_conv3x3_narrow_fwd(
+                x.data_ptr(), tc_conv.nhwc_geometry(x)[4], wl.data_ptr(), b.data_ptr() if b is not None else None,
+                y.data_ptr(), 4, N, H, W, C, 2, torch.cuda.current_stream().cuda_stream), "conv3x3_narrow_fwd")
         ctx.save_for_backward(x, w)
         ctx.has_b = b is not None
         ctx.gen = _generation
@@ -597,24 +412,19 @@ class _NarrowConv3x3(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, g):
+        from . import tc_conv
         x, w = ctx.saved_tensors
         N, C, H, W = x.shape
         gx = gw = gb = None
         if ctx.needs_input_grad[0]:
-            from . import tc_conv
-            if _TC and tc_conv.supported(x):
-                # input gradient (C_in wide) on the tensor-core kernel: contraction over the 2 flow channels
-                gd, _ = _lrelu_bwd_bias(g, None, False)
-                gx = _input_grad_into_slot(ctx.gen, x, lambda dst, acc: tc_conv.run(
-                    gd, tc_conv.split_weights(_khwc(w), transpose=True), dst, mode=1, stride=1, kh=3, kw=3,
-                    pad_t=1, pad_l=1, accumulate=acc))
-            else:
-                ci_p = _round4(C)
-                gs = _operand(g, 0, c_pad=4)                                          # [N, 12, H, W]
-                wt = _operand(w, 1, concat_batch=True, c_pad=ci_p, n_out=4)           # [12, Ci_p, 3, 3]
-                gx = _conv_input_grad((H + 2, W + 2), wt, gs, 1)[:, :C, 1:1 + H, 1:1 + W]
+            # contraction over the 2 flow channels; the launch reads only the gradient, so x's pitch does not
+            # matter: dL/dx goes to a fresh round4-pitched buffer or a registered gradient slot
+            gd, _ = _lrelu_bwd_bias(g, None, False)
+            gx = _input_grad_into_slot(ctx.gen, x, lambda dst, acc: tc_conv.run(
+                gd, tc_conv.split_weights(_khwc(w), transpose=True), dst, mode=1, stride=1, kh=3, kw=3,
+                pad_t=1, pad_l=1, accumulate=acc))
         if ctx.needs_input_grad[1]:
-            lib = _narrow_lib()
+            lib = _native.lib()
             ws = torch.empty(lib.unflow_conv3x3_narrow_wgrad_workspace_bytes(N, H, W, C) // 4,
                              device=x.device, dtype=torch.float32)
             gw = torch.empty((2, 3, 3, C), device=x.device, dtype=torch.float32)
@@ -622,8 +432,8 @@ class _NarrowConv3x3(torch.autograd.Function):
             from ..ops import kernel_timer
             with torch.cuda.device(x.device), kernel_timer.span("narrow_conv_wgrad", 4 * x.numel() + 4 * g.numel()):
                 check(lib.unflow_conv3x3_narrow_wgrad(
-                    x.data_ptr(), _pixel_pitch(x), g.data_ptr(), sN, sC, sH, sW, gw.data_ptr(), ws.data_ptr(),
-                    N, H, W, C, 2, torch.cuda.current_stream().cuda_stream), "conv3x3_narrow_wgrad")
+                    x.data_ptr(), tc_conv.nhwc_geometry(x)[4], g.data_ptr(), sN, sC, sH, sW, gw.data_ptr(),
+                    ws.data_ptr(), N, H, W, C, 2, torch.cuda.current_stream().cuda_stream), "conv3x3_narrow_wgrad")
             gw = gw.permute(0, 3, 1, 2)                                           # [2, C, 3, 3], NHWC-ordered
         if ctx.has_b and ctx.needs_input_grad[2]:
             gb = _bias_grad(g, None)
@@ -636,11 +446,10 @@ class _NarrowConv3x3(torch.autograd.Function):
 # channels -- 2x2 pixel blocks become 4*C channels, the 7x7 filter (zero-extended to 8x8) a 4x4
 # filter with stride 1 -- is the same sum with a tensor-core-friendly shape (4*C*3 = 36 channels).
 S2D_MAX_CHANNELS = 16
-_S2D = __import__('os').environ.get('UNFLOW_CONV1_S2D', '1') != '0'
 
 
 def _use_space_to_depth(x, w, stride):
-    return (_S2D and stride in (2, (2, 2)) and w.shape[2] == w.shape[3] and w.shape[2] % 2 == 1
+    return (stride in (2, (2, 2)) and w.shape[2] == w.shape[3] and w.shape[2] % 2 == 1
             and w.shape[2] >= 5 and w.shape[1] <= S2D_MAX_CHANNELS)
 
 
@@ -662,31 +471,27 @@ def space_to_depth_operands(x, w, pads):
     return xs, ws
 
 
-def channels_last_active(x):
-    """The tensor-core path computes in NHWC (cuDNN's TF32 kernels are NHWC; NCHW costs a layout
-    transform around every conv); the exact-fp32 path keeps the reference's NCHW (cuDNN's fp32
-    NHWC kernels measured 18 % slower than NCHW on this network)."""
-    return _MODE != 'fp32' and x.is_cuda
+def tc_active(x):
+    """True when the layers fed ``x`` run on the tensor-core kernels (3xTF32 mode, CUDA tensors).  They
+    compute in NHWC: the network input is then a free view of the NHWC images, concats go into NHWC
+    buffers, and callers may hand ``out=`` slots (channel slices of pre-allocated concat buffers) to
+    conv2d / conv_transpose2d.  The exact-fp32 path keeps the reference's NCHW (cuDNN's fp32 NHWC kernels
+    measured 18 % slower than NCHW on this network)."""
+    return _MODE == '3xtf32' and x.is_cuda
 
 
 def network_input(x_nhwc):
     """NHWC image batch -> the NCHW-shaped tensor the conv stack consumes.  In the tensor-core
     mode this is a free view (NHWC memory == channels_last); in fp32 mode an NCHW copy."""
     x = x_nhwc.permute(0, 3, 1, 2)
-    return x if channels_last_active(x_nhwc) else x.contiguous()
-
-
-def direct_write_ok(x):
-    """True when the tensor-core layers are active, i.e. when a caller may hand ``out=`` slots (channel
-    slices of pre-allocated concat buffers) to conv2d / conv_transpose2d."""
-    return _TC and _MODE == '3xtf32' and x.is_cuda
+    return x if tc_active(x_nhwc) else x.contiguous()
 
 
 def conv2d(x, w, b, stride, pads, act=False, out=None):
     """pads = (top, bottom, left, right) TF-SAME padding; act: apply the leaky ReLU.  ``out``: optional
     destination (NCHW-shaped view with NHWC memory); honoured by the tensor-core path -- the result then
     aliases it -- and ignored by the others (the caller's concat copies as before)."""
-    if _MODE == '3xtf32' and x.is_cuda:
+    if tc_active(x):
         if not act and _use_narrow(x, w, stride, pads):
             return _NarrowConv3x3.apply(x, w, b)
         if _use_window(x, w, stride):
@@ -696,31 +501,30 @@ def conv2d(x, w, b, stride, pads, act=False, out=None):
         if _use_space_to_depth(x, w, stride):
             xs, ws = space_to_depth_operands(x, w, pads)
             return conv2d(xs, ws, b, 1, (0, 0, 0, 0), act=act)
-        if _tc_ok(x, stride) and w.shape[2] == w.shape[3] and w.shape[2] * w.shape[3] <= 64:
-            return _ConvTC.apply(x, w, b, stride, tuple(pads), bool(act), out)
-        fuse = act and b is not None and w.shape[0] % 4 == 0
-        y = _Conv3x.apply(x, w, b, stride, tuple(pads), fuse)
-        return F.leaky_relu(y, LRELU_SLOPE) if (act and not fuse) else y
+        kh, kw = w.shape[2], w.shape[3]
+        if kh != kw or kh * kw > 64 or kh < stride:
+            # (k < stride: the input gradient's transposed launch would have output parity classes without a tap)
+            raise ValueError("the tensor-core conv takes square k x k filters with stride <= k <= 8, not %dx%d at "
+                             "stride %d" % (kh, kw, stride))
+        x, pads = _tc_input(x, stride, pads)
+        return _ConvTC.apply(x, w, b, stride, tuple(pads), bool(act), out)
     pt, pb, pl, pr = pads
     if pt == pb and pl == pr:
         padding = (pt, pl)
     else:
         x = F.pad(x, (pl, pr, pt, pb))
         padding = (0, 0)
-    if x.is_cuda and _MODE == 'fp32':
+    if x.is_cuda:
         w = w.contiguous()     # parameters are stored NHWC-ordered; the exact-fp32 path computes in NCHW
     y = F.conv2d(x, w, b, stride=stride, padding=padding)
     return F.leaky_relu(y, LRELU_SLOPE) if act else y
 
 
 def conv_transpose2d(x, w, b, act=False, out=None):
-    if _MODE == '3xtf32' and x.is_cuda:
-        if _tc_ok(x, 1):
-            return _DeconvTC.apply(x, w, b, bool(act), out)
-        fuse = act and b is not None and w.shape[1] % 4 == 0
-        y = _Deconv3x.apply(x, w, b, fuse)
-        return F.leaky_relu(y, LRELU_SLOPE) if (act and not fuse) else y
-    if x.is_cuda and _MODE == 'fp32':
+    if tc_active(x):
+        x, _ = _tc_input(x)
+        return _DeconvTC.apply(x, w, b, bool(act), out)
+    if x.is_cuda:
         w = w.contiguous()
     y = F.conv_transpose2d(x, w, b, stride=2, padding=1)
     return F.leaky_relu(y, LRELU_SLOPE) if act else y

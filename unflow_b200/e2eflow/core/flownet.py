@@ -34,8 +34,8 @@ def set_conv_precision(mode='fp32'):
     'fp32' (default): exact float32 cuDNN convolutions, what the reference's TF1 graph computes.
     torch enables single-pass TF32 convolutions by default, which costs ~1e-3 relative on the flow
     fields and breaks the 1e-4 parity bar (measured) -- so it is switched off on import.
-    '3xtf32': tensor-core convolutions at fp32-level accuracy (operand split, one fused conv).
-    'tf32': single-pass TF32, an explicitly reduced-precision mode."""
+    '3xtf32': convolutions on the hand-written tensor-core kernels at fp32-level accuracy (every operand
+    split into TF32 hi + lo, three products accumulated in fp32)."""
     return conv_ops.set_mode(mode)
 
 
@@ -294,7 +294,7 @@ class _Cat:
 def _decoder_cats(s, like, n, hw3, hw2, c2):
     """Concat buffers of _flownet_upconv for a trunk whose conv3_1 is ``hw3`` and whose conv2 (``c2``
     channels) is ``hw2`` in size; None when the tensor-core path is not active for ``like``."""
-    if not conv_ops.direct_write_ok(like):
+    if not conv_ops.tc_active(like):
         return None
     half = lambda v: -(-v // 2)
     (h3, w3), (h2, w2) = hw3, hw2
@@ -470,7 +470,7 @@ def _concat_channels_last(first, second_batch_parts=None, buf=None):
 
 def _cat_c(tensors, buf=None):
     """tf.concat(tensors, 1) of NCHW-shaped tensors (``buf``: pre-allocated NHWC destination, see _Cat)."""
-    if conv_ops.channels_last_active(tensors[0]):
+    if conv_ops.tc_active(tensors[0]):
         return _concat_channels_last(list(tensors), buf=buf)
     return torch.cat(tensors, 1)
 
@@ -484,9 +484,10 @@ def _trunk_input_bidir(cs, conv3_ab, kw):
     correlation_bidir_concat).  None when the tiled correlation kernel does not serve the shape."""
     from ..ops import correlation_bidir_concat, _corr_attrs
     from ... import _native
+    from . import tc_conv
     n2, C, H, W = conv3_ab.shape
     attrs = _corr_attrs(kw)
-    if n2 % 2 or _native.lib().unflow_correlation_fwd_path(C, H, W, *attrs) != 1 or not conv_ops._tc_ok(conv3_ab, 1):
+    if n2 % 2 or _native.lib().unflow_correlation_fwd_path(C, H, W, *attrs) != 1 or not tc_conv.supported(conv3_ab):
         return None
     md, s2 = attrs[1], attrs[4]
     D = (2 * (md // s2) + 1) ** 2
@@ -504,7 +505,7 @@ def flownet_c(conv3_a, conv3_b, conv2_a, channel_mult=1, full_res=False, _scope=
     corr = correlation(conv3_a, conv3_b,
                        pad=20, kernel_size=1, max_displacement=20, stride_1=1, stride_2=2)
     conv_redir = s.conv(conv3_a, 'conv_redir')
-    if conv_ops.channels_last_active(conv_redir):
+    if conv_ops.tc_active(conv_redir):
         trunk_in = _concat_channels_last([conv_redir], [corr])
     else:
         trunk_in = torch.cat([conv_redir, corr], 1)
@@ -548,7 +549,7 @@ def flownet(im1, im2, flownet_spec='S', full_resolution=False, train_all=False,
                 conv3_a, conv3_b = conv3_ab[:B], conv3_ab[B:]
                 kw = dict(pad=20, kernel_size=1, max_displacement=20, stride_1=1, stride_2=2)
                 trunk_in = (_trunk_input_bidir(cs, conv3_ab, kw)
-                            if FUSED_TRUNK_INPUT and conv_ops.direct_write_ok(conv3_ab) else None)
+                            if FUSED_TRUNK_INPUT and conv_ops.tc_active(conv3_ab) else None)
                 if trunk_in is not None:
                     pass        # conv_redir and both cost volumes written into one NHWC buffer (ops.py)
                 else:
@@ -558,7 +559,7 @@ def flownet(im1, im2, flownet_spec='S', full_resolution=False, train_all=False,
                     else:   # (CPU: only reachable with the op swapped for a stand-in, as the host-logic tests do)
                         corr_ab, corr_ba = correlation(conv3_a, conv3_b, **kw), correlation(conv3_b, conv3_a, **kw)
                     conv_redir = cs.conv(conv3_ab, 'conv_redir')
-                    if conv_ops.channels_last_active(conv_redir):
+                    if conv_ops.tc_active(conv_redir):
                         trunk_in = _concat_channels_last([conv_redir], [corr_ab, corr_ba])
                     else:
                         trunk_in = torch.cat([conv_redir, torch.cat([corr_ab, corr_ba], 0)], 1)
