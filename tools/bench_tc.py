@@ -12,6 +12,8 @@ operands still alive, replayed alone with the same pointers and shapes:
 
   * plan: BN, tiles and work items from unflow_tc_conv_plan / unflow_tc_wgrad_plan.  For conv the K slices are
     those the launcher uses for this call's epilogue; for wgrad the K blocks per item and the chunks along K.
+    Schedule (csrc/tc_schedule.h): items / 132 SMs (waves), the items run whole in round robin (DP), the items
+    of the stream-K tail (SK) and the segments the tail is cut into over the grid (SK 0: plain round robin).
   * time: R launches captured in a CUDA graph, replayed K times between CUDA events; the median replay / R.
     TF32 share as bench.py counts it: 3 MMA passes x nominal flops (2 x multiply-adds of the fp32 product)
     over the data-sheet TF32 rate (989 / 2 TFLOP/s, H100 SXM, a 700 W card).
@@ -47,17 +49,87 @@ from float64_refs import view  # noqa: E402
 from unflow_b200 import synthetic as synth  # noqa: E402
 
 TF32_TFLOPS = 989.0 / 2          # H100 SXM data sheet, dense: bf16 / 2
+GRID = 132                       # CTAs of a tc launch (one per SM)
+CHUNK = 8                        # K blocks per accumulation chunk (tc_chunk default): the stream-K cut unit
+
+
 ENTRY_POINTS = {"conv": ("unflow_tc_conv", "unflow_tc_conv_window"),
                 "wgrad": ("unflow_tc_wgrad", "unflow_tc_wgrad_window")}
 PLANS = ("unflow_tc_conv_plan", "unflow_tc_wgrad_plan", "unflow_tc_conv_debug")
+SPLIT_COST = 1                   # csrc/tc_schedule.h: kSkSplitCost, chunks per segment of a split item
+
+
+def schedule(lengths, grid=GRID, chunk=CHUNK):
+    """(DP items, SK items, SK segments) of make_sk_schedule (csrc/tc_schedule.h) for items of these K lengths;
+    (items, 0, 0) where the launch stays round robin."""
+    T = len(lengths)
+    rr = [0] * grid
+    for i, L in enumerate(lengths):
+        rr[i % grid] += L
+    waves = T // grid
+    dp = (waves - 1 if T % grid and waves else waves) * grid
+    sk = lengths[dp:]
+    if not sk:
+        return T, 0, 0
+    load = [0] * grid
+    for i in range(dp):
+        load[i % grid] += lengths[i]
+    total = sum(sk)
+    lo, hi = 0, max(load) + total
+    while lo < hi:
+        mid = (lo + hi) // 2
+        if sum(max(0, mid - d) for d in load) >= total:
+            hi = mid
+        else:
+            lo = mid + 1
+    room_all = sum(max(0, lo - d) for d in load)
+    bounds, j, off, room = [], 0, 0, 0
+    for g in range(grid + 1):
+        if g:
+            room += max(0, lo - load[g - 1])
+        target = total if g == grid else total * room // room_all
+        while j < len(sk) and off + sk[j] <= target:
+            off += sk[j]
+            j += 1
+        if j == len(sk):
+            bounds.append((len(sk), 0))
+            continue
+        k = -(-(target - off) // chunk) * chunk
+        bounds.append((j, k) if k < sk[j] else (j + 1, 0))
+    segs, span = 0, 0
+    for g, ((j0, k0), (je, ke)) in enumerate(zip(bounds, bounds[1:])):
+        cta = load[g]
+        for jj in range(j0, min(je, len(sk) - 1) + 1):
+            a, b = (k0 if jj == j0 else 0), (ke if jj == je else sk[jj])
+            if b <= a:
+                continue
+            segs += 1
+            cta += b - a + (SPLIT_COST * chunk if a > 0 or b < sk[jj] else 0)
+        span = max(span, cta)
+    if span + chunk > max(rr):
+        return T, 0, 0
+    return dp, len(sk), segs
 
 
 def conv_plan(lib, plan_args):
-    """(BN, tiles, n_classes, n_blocks, K slices when the epilogue allows slicing) of unflow_tc_conv_plan."""
+    """(BN, tiles, n_classes, n_blocks, K slices when the epilogue allows slicing, K blocks per class) of
+    unflow_tc_conv_plan."""
     buf = (ctypes.c_int * 1024)()
     n = lib.unflow_tc_conv_plan(*plan_args, buf, 1024)
     assert n > 0, n
-    return buf[12], buf[8] * buf[9] * buf[10], buf[0], buf[11], buf[n - 1]
+    cs = list(buf[15:16 + buf[0]])
+    return buf[12], buf[8] * buf[9] * buf[10], buf[0], buf[11], buf[n - 1], [(b - a) * buf[13] for a, b in zip(cs, cs[1:])]
+
+
+def conv_lengths(tiles, ncls, nblk, ks, class_k):
+    """K blocks of each work item in the kernel's order (csrc/tc_conv.cu: decode_work)."""
+    out = []
+    for w in range(tiles * ncls * nblk * ks):
+        tile, s = divmod(w, ks)
+        total = class_k[(tile // nblk) % ncls]
+        per = -(-total // ks)
+        out.append(max(0, min(per, total - s * per)))
+    return out
 
 
 def geometry(lib, name, a):
@@ -66,8 +138,8 @@ def geometry(lib, name, a):
     if name == "unflow_tc_conv":
         (_, N, Hin, Win, Cin, _, _, _, y, Hout, Wout, Cout, y_pitch, bias, _, act, accumulate, mode, stride, kh, kw,
          pad_t, pad_l, _) = a
-        BN, tiles, ncls, nblk, ks = conv_plan(lib, (N, Hin, Win, Cin, Hout, Wout, Cout, mode | 4, stride, kh, kw,
-                                                    pad_t, pad_l))
+        BN, tiles, ncls, nblk, ks, class_k = conv_plan(lib, (N, Hin, Win, Cin, Hout, Wout, Cout, mode | 4, stride, kh,
+                                                             kw, pad_t, pad_l))
         # the launcher's rule (csrc/tc_conv.cu, unflow_tc_conv): slice only where the epilogue allows it
         if not ((not bias and not act) or (bias and act and not accumulate and y_pitch == Cout and Cout % 4 == 0)):
             ks = 1
@@ -75,13 +147,16 @@ def geometry(lib, name, a):
         row = dict(kind="deconv" if mode == 1 else "conv", acc=bool(accumulate), taps="%d/%d" % (kh * kw, stride),
                    shape="%dx%dx%dx%d>%dx%dx%d" % (N, Hin, Win, Cin, Hout, Wout, Cout),
                    BN=BN, ksplit=ks, items=tiles * ncls * nblk * ks)
+        row["dp"], row["sk"], row["sk_segments"] = schedule(conv_lengths(tiles, ncls, nblk, ks, class_k))
         return y, (N * Hout * Wout - 1) * y_pitch + Cout, 2 * pix * Cout * Cin * kh * kw, row, ks > 1
     if name == "unflow_tc_conv_window":
         _, N, H, _, Cp, _, _, y, Hout, Wout, Cout, y_pitch, _, _, _, kh, stride, pad_t, _ = a
-        BN, tiles, ncls, nblk, _ = conv_plan(lib, (N, H, Wout, 8 * Cp, Hout, Wout, Cout, 0, stride, kh, 1, pad_t, 0))
+        BN, tiles, ncls, nblk, _, class_k = conv_plan(lib, (N, H, Wout, 8 * Cp, Hout, Wout, Cout, 0, stride, kh, 1,
+                                                            pad_t, 0))
         row = dict(kind="window", acc=False, taps="%d/%d" % (kh, stride),
                    shape="%dx%dx%dx%d>%dx%dx%d" % (N, H, Wout, 8 * Cp, Hout, Wout, Cout),
                    BN=BN, ksplit=1, items=tiles * ncls * nblk)
+        row["dp"], row["sk"], row["sk_segments"] = schedule(conv_lengths(tiles, ncls, nblk, 1, class_k))
         return y, (N * Hout * Wout - 1) * y_pitch + Cout, 2 * N * Hout * Wout * Cout * 8 * Cp * kh, row, False
     if name == "unflow_tc_wgrad":
         _, N, Hp, Wp, R, _, _, _, _, C, _, dw, pitch_r, _, stride, kh, kw, pad_t, pad_l, _ = a
@@ -95,6 +170,8 @@ def geometry(lib, name, a):
     assert lib.unflow_tc_wgrad_plan(*plan, v) == 15
     row = dict(kind=kind, taps="%d/%d" % (taps, stride), shape="%dx%dx%d, %dx%d" % (plan[:5]),
                BN=v[11], kc=v[7], n_chunks=v[8], items=v[8] * v[9] * v[10])
+    row["dp"], row["sk"], row["sk_segments"] = schedule(
+        [min(v[7], v[6] - c * v[7]) for c in range(v[8]) for _ in range(v[9] * v[10])])
     return dw, n_dw, flops, row, v[8] > 1
 
 
@@ -199,24 +276,25 @@ class Bench:
 
 
 HEAD = {
-    "conv": "%3s %-6s %-3s %-26s %-6s %4s %3s %5s %6s %8s %6s %6s %6s" % (
-        "#", "kind", "acc", "N x Hin x Win x Cin>out", "taps/s", "BN", "ks", "items", "stages", "us", "tf32",
-        "c.full", "p.empt"),
-    "wgrad": "%3s %-6s %-22s %-7s %4s %3s %3s %5s %6s %8s %6s %6s %6s %6s" % (
-        "#", "kind", "N x Hp x Wp, R x C", "taps/s", "BN", "kc", "ch", "items", "stages", "us", "tf32",
-        "c.full", "p.empt", "c.splt"),
+    "conv": "%3s %-6s %-3s %-26s %-6s %4s %3s %5s %6s %5s %5s %5s %6s %8s %6s %6s %6s" % (
+        "#", "kind", "acc", "N x Hin x Win x Cin>out", "taps/s", "BN", "ks", "items", "waves", "DP", "SK", "segs",
+        "stages", "us", "tf32", "c.full", "p.empt"),
+    "wgrad": "%3s %-6s %-22s %-7s %4s %3s %3s %5s %6s %5s %5s %5s %6s %8s %6s %6s %6s %6s" % (
+        "#", "kind", "N x Hp x Wp, R x C", "taps/s", "BN", "kc", "ch", "items", "waves", "DP", "SK", "segs",
+        "stages", "us", "tf32", "c.full", "p.empt", "c.splt"),
 }
 
 
 def fmt(kernel, i, r):
     st = "+".join("%d" % x for x in r["stages"]) if r["stages"] else "-"
     if kernel == "conv":
-        line = "%3d %-6s %-3s %-26s %-6s %4d %3d %5d %6s %8.1f %5.1f%% %5.1f%% %5.1f%%" % (
-            i, r["kind"], "+=" if r["acc"] else "", r["shape"], r["taps"], r["BN"], r["ksplit"], r["items"], st,
-            r["us"], 100 * r["tf32_share"], 100 * r["cons_full_wait"], 100 * r["prod_empty_wait"])
+        line = "%3d %-6s %-3s %-26s %-6s %4d %3d %5d %6.2f %5d %5d %5d %6s %8.1f %5.1f%% %5.1f%% %5.1f%%" % (
+            i, r["kind"], "+=" if r["acc"] else "", r["shape"], r["taps"], r["BN"], r["ksplit"], r["items"],
+            r["items"] / GRID, r["dp"], r["sk"], r["sk_segments"], st, r["us"], 100 * r["tf32_share"], 100 * r["cons_full_wait"], 100 * r["prod_empty_wait"])
     else:
-        line = "%3d %-6s %-22s %-7s %4d %3d %3d %5d %6s %8.1f %5.1f%% %5.1f%% %5.1f%% %6s" % (
-            i, r["kind"], r["shape"], r["taps"], r["BN"], r["kc"], r["n_chunks"], r["items"], st, r["us"],
+        line = "%3d %-6s %-22s %-7s %4d %3d %3d %5d %6.2f %5d %5d %5d %6s %8.1f %5.1f%% %5.1f%% %5.1f%% %6s" % (
+            i, r["kind"], r["shape"], r["taps"], r["BN"], r["kc"], r["n_chunks"], r["items"], r["items"] / GRID,
+            r["dp"], r["sk"], r["sk_segments"], st, r["us"],
             100 * r["tf32_share"], 100 * r["cons_full_wait"], 100 * r["prod_empty_wait"],
             "-" if r["cons_split_wait"] is None else "%.1f%%" % (100 * r["cons_split_wait"]))
     c = r["compare"]

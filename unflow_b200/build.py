@@ -33,7 +33,7 @@ def needs_build():
     if not os.path.exists(LIB):
         return True
     t = os.path.getmtime(LIB)
-    deps = sources() + [os.path.join(CSRC, f) for f in os.listdir(CSRC) if f.endswith(".cuh")]
+    deps = sources() + [os.path.join(CSRC, f) for f in os.listdir(CSRC) if f.endswith((".cuh", ".h"))]
     deps.append(os.path.join(os.path.dirname(HERE), "include", "unflow.h"))
     return any(os.path.getmtime(d) > t for d in deps)
 

@@ -4,9 +4,12 @@
 #include <cuda.h>
 
 #include "common.cuh"
+#include "tc_schedule.h"
 
 namespace unflow {
 namespace tc {
+
+static_assert(kNumSMs <= kSkMaxGrid, "the stream-K schedule holds one range per SM");
 
 constexpr int BM = 128;          // rows of a tile: two consumer warpgroups of 64 rows (the wgmma M)
 constexpr int BK = 32;           // fp32 elements per K block = 128 bytes = one swizzle row
@@ -172,6 +175,38 @@ template <> struct Wgmma<128> {
         : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(scale_d));
   }
 };
+
+// ---- the segments a CTA runs (tc_schedule.h) ---------------------------------------------------------------
+// The producer warp and the consumers of a CTA walk the same list: the first n_dp segments are the DP items
+// blockIdx.x, blockIdx.x + grid, ..., whole; the rest are the pieces of the CTA's SK range, one per item it touches.
+struct Segment {
+  int item, k0, k1;      // item and its K blocks [k0, k1); k1 < 0: to the item's end
+  int sk;                // SK item index (item - dp_items), or -1 for a DP item
+};
+struct SegmentWalk {
+  int n_dp, n_seg;
+};
+__device__ __forceinline__ SegmentWalk segment_walk(const SkSchedule &s) {
+  const int g = blockIdx.x;
+  const int j0 = s.sk_item[g], k0 = s.sk_k[g], je = s.sk_item[g + 1], ke = s.sk_k[g + 1];
+  SegmentWalk w;
+  w.n_dp = g < s.dp_items ? (s.dp_items - g + (int)gridDim.x - 1) / (int)gridDim.x : 0;
+  w.n_seg = w.n_dp + (j0 == je ? (ke > k0 ? 1 : 0) : je - j0 + (ke > 0 ? 1 : 0));
+  return w;
+}
+__device__ __forceinline__ Segment segment_at(const SkSchedule &s, const SegmentWalk &w, int q) {
+  Segment sg;
+  const int g = blockIdx.x;
+  if (q < w.n_dp) {
+    sg.item = g + q * (int)gridDim.x; sg.k0 = 0; sg.k1 = -1; sg.sk = -1;
+    return sg;
+  }
+  const int j = s.sk_item[g] + (q - w.n_dp);
+  sg.sk = j; sg.item = s.dp_items + j;
+  sg.k0 = q == w.n_dp ? s.sk_k[g] : 0;
+  sg.k1 = j == s.sk_item[g + 1] ? s.sk_k[g + 1] : -1;
+  return sg;
+}
 
 // ---- host: tensor maps --------------------------------------------------------------------------
 typedef CUresult (*EncodeTiledFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *,

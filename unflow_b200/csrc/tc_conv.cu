@@ -39,6 +39,10 @@
 // The activations are read from HBM once, as fp32; no [hi,hi,lo] operand copies exist, no layout
 // conversion, no separate bias / activation pass.
 //
+// Schedule (tc_schedule.h): whole work items round robin for all but the last one or two waves; the K blocks of
+// the rest are spread over the grid so that every CTA ends at the same time (where that shortens the launch), and
+// a tile run by several CTAs is finished by the warp that completes it last (sk_fixup).
+//
 // Accuracy: hi carries 11 significant bits, lo the next 11; the dropped lo*lo' term and the
 // truncation of lo are ~2^-22 relative.  What limits a long tensor-core accumulation is not the
 // split but the accumulator itself: the MMA adds with truncation, a bias of a fraction of an ulp
@@ -81,6 +85,9 @@ struct ConvParams {
   int class_start[5];
   short class_px[4], class_py[4];
   Tap taps[MAX_TAPS];
+  SkSchedule sk;              // the segments of each CTA (tc_schedule.h)
+  float *sk_part;             // stream-K fixup: partial sums of split tiles, 2 slots per CTA (see sk_storage)
+  unsigned *sk_count;         // stream-K fixup: arrivals per SK item and consumer warp, zero between launches
 };
 
 // Stage: [A raw fp32] [B hi] [B lo].  Each 1024-byte aligned (128-byte swizzle atoms).  The ring fills the opt-in
@@ -128,16 +135,77 @@ struct Work {
   TileCoord t;
   int it0, iters;       // first K block (tap * kblocks + channel block) and count of this item
 };
+__device__ __host__ __forceinline__ void work_range(const ConvParams &p, int cls, int ks, int &it0, int &iters) {
+  const int total = (p.class_start[cls + 1] - p.class_start[cls]) * p.kblocks;
+  const int per = (total + p.ksplit - 1) / p.ksplit;
+  it0 = ks * per;
+  iters = total - it0 < per ? total - it0 : per;
+  if (iters < 0) iters = 0;
+}
 __device__ __forceinline__ Work decode_work(const ConvParams &p, int w) {
   Work k;
   const int tile = w / p.ksplit, ks = w - tile * p.ksplit;
   k.t = decode_tile(p, tile);
-  const int total = (p.class_start[k.t.cls + 1] - p.class_start[k.t.cls]) * p.kblocks;
-  const int per = (total + p.ksplit - 1) / p.ksplit;
-  k.it0 = ks * per;
-  k.iters = total - k.it0 < per ? total - k.it0 : per;
-  if (k.iters < 0) k.iters = 0;
+  work_range(p, k.t.cls, ks, k.it0, k.iters);
   return k;
+}
+// K blocks of work item w (the schedule's item length)
+__device__ __host__ __forceinline__ int work_len(const ConvParams &p, int w) {
+  const int tile = w / p.ksplit, ks = w - tile * p.ksplit;
+  int it0, iters;
+  work_range(p, (tile / p.n_blocks) % p.n_classes, ks, it0, iters);
+  return iters;
+}
+
+// Stream-K fixup of a tile that several CTAs run one K range each (tc_schedule.h).  Bias, leaky ReLU and += are
+// not linear in the partial sums, so one of them has to see the whole sum.  Per consumer warp (a warp owns 16 rows
+// of the tile and nothing else): every segment stores its partial to its slot -- 2g for the first segment of CTA g,
+// 2g + 1 for its last -- then, after a warp barrier, one lane counts the warp on the item's counter with an
+// acq_rel atomic (release: the warp's stores are visible before the count; acquire: the last arriver sees every
+// other partial).  The warp that completes the count adds all partials in segment order (a fixed order: the result
+// does not depend on who arrives last), resets the counter for the next launch and runs the epilogue.  No CTA waits
+// for another.
+__device__ __forceinline__ unsigned atom_add_acq_rel(unsigned *addr, unsigned v) {
+  unsigned old;
+  asm volatile("atom.acq_rel.gpu.global.add.u32 %0, [%1], %2;" : "=r"(old) : "l"(addr), "r"(v) : "memory");
+  return old;
+}
+template <int R>
+__device__ __forceinline__ bool sk_fixup(const ConvParams &p, const Segment &sg, int len, int cwarp, int lane,
+                                         float (&sum)[R]) {
+  const SkSchedule &s = p.sk;
+  const int g = blockIdx.x, j = sg.sk;
+  auto slot_of = [&](int c) { return 2 * c + (s.sk_item[c] == j ? 0 : 1); };
+  auto part = [&](int slot) { return p.sk_part + ((long long)(slot * 8 + cwarp) * R) * 32 + lane; };
+  {
+    float *dst = part(slot_of(g));
+#pragma unroll
+    for (int c = 0; c < R; ++c) __stcg(dst + 32 * c, sum[c]);
+  }
+  __syncwarp();
+  // the CTAs whose ranges meet item j: ga holds its first K block, gb its last; empty ranges in between run nothing
+  int ga = g, gb = g;
+  while (ga > 0 && (s.sk_item[ga] > j || (s.sk_item[ga] == j && s.sk_k[ga] > 0))) --ga;
+  while (s.sk_item[gb + 1] < j || (s.sk_item[gb + 1] == j && s.sk_k[gb + 1] < len)) ++gb;
+  auto empty = [&](int c) { return s.sk_item[c] == s.sk_item[c + 1] && s.sk_k[c] == s.sk_k[c + 1]; };
+  unsigned n = 0;
+  for (int c = ga; c <= gb; ++c) n += empty(c) ? 0u : 1u;
+  unsigned *cnt = p.sk_count + 8 * j + cwarp;
+  unsigned old = 0;
+  if (lane == 0) old = atom_add_acq_rel(cnt, 1u);
+  old = __shfl_sync(0xffffffffu, old, 0);
+  if (old != n - 1) return false;
+  __syncwarp();                                 // lane 0's acquire before every lane's loads
+  if (lane == 0) *cnt = 0u;
+#pragma unroll
+  for (int c = 0; c < R; ++c) sum[c] = 0.f;
+  for (int c = ga; c <= gb; ++c) {
+    if (empty(c)) continue;
+    const float *src = part(slot_of(c));
+#pragma unroll
+    for (int e = 0; e < R; ++e) sum[e] += __ldcg(src + 32 * e);
+  }
+  return true;
 }
 
 // ------------------------------------------------------------------------------------------
@@ -159,8 +227,6 @@ tc_conv_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
   // warp index made warp-uniform for ptxas: with a plain threadIdx.x >> 5 it cannot prove the role branch is uniform
   // across a warpgroup, treats the wgmma code as divergent and waits for every MMA before issuing the next (C7518)
   const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0), lane = threadIdx.x & 31;
-  const int m_tiles = p.tiles_n * p.tiles_y * p.tiles_x;
-  const int total_items = p.n_classes * m_tiles * p.n_blocks * p.ksplit;
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < C::STAGES; ++s) {
@@ -183,12 +249,15 @@ tc_conv_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
     unsigned ph = 0;
     long long t_wait = 0, t_all = clock64();          // role timers: cycles blocked on the barrier / in total
     const unsigned a_box_bytes = (unsigned)(p.TW * p.TH * p.TN) * BK * 4u;
-    for (int item = blockIdx.x; item < total_items; item += gridDim.x) {
-      const Work wk = decode_work(p, item);
+    const SegmentWalk walk = segment_walk(p.sk);
+    for (int q = 0; q < walk.n_seg; ++q) {
+      const Segment sg = segment_at(p.sk, walk, q);
+      const Work wk = decode_work(p, sg.item);
       const TileCoord t = wk.t;
       const int x0 = p.s_in_x * t.ix0, y0 = p.s_in_y * t.iy0;
-      int ti = p.class_start[t.cls] + wk.it0 / p.kblocks, kc = wk.it0 % p.kblocks;
-      for (int it = 0; it < wk.iters; ++it) {
+      int ti = p.class_start[t.cls] + (wk.it0 + sg.k0) / p.kblocks, kc = (wk.it0 + sg.k0) % p.kblocks;
+      const int k1 = sg.k1 < 0 ? wk.iters : sg.k1;
+      for (int it = sg.k0; it < k1; ++it) {
         const Tap tap = p.taps[ti];
         { const long long t0 = clock64(); mbar_wait(empty(s), ph ^ 1u); t_wait += clock64() - t0; }
         const unsigned st = base + s * C::STAGE_BYTES;
@@ -225,10 +294,13 @@ tc_conv_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
     long long t_wait = 0, t_all = clock64();
     float sum[R], acc[R];
     unsigned a_hi[FRAG_SETS][4], a_lo[FRAG_SETS][4];
-    for (int item = blockIdx.x; item < total_items; item += gridDim.x) {
-      const Work wk = decode_work(p, item);
+    const SegmentWalk walk = segment_walk(p.sk);
+    for (int q = 0; q < walk.n_seg; ++q) {
+      // a segment starts on a chunk boundary of its item: its chunks are the item's chunks
+      const Segment sg = segment_at(p.sk, walk, q);
+      const Work wk = decode_work(p, sg.item);
       const TileCoord t = wk.t;
-      const int iters = wk.iters;
+      const int k1 = sg.k1 < 0 ? wk.iters : sg.k1, iters = k1 - sg.k0;
 #pragma unroll
       for (int c = 0; c < R; ++c) sum[c] = 0.f;
       // Outer loop over chunks, inner loop over the K blocks of a chunk.  Inside a chunk the only waits are
@@ -280,6 +352,11 @@ tc_conv_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
 #pragma unroll
         for (int c = 0; c < R; ++c) sum[c] += acc[c];
       }
+      // a tile split over CTAs: only the last warp to finish its part goes on, with the whole sum (K slices add
+      // their parts with red.add anyway)
+      if (p.ksplit == 1 && sg.sk >= 0 && (sg.k0 > 0 || k1 < wk.iters) &&
+          !sk_fixup(p, sg, wk.iters, warp - 4, lane, sum))
+        continue;
       // ---- epilogue: rows row0 and row0 + 8, columns 8j + col0 (+1) ----
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
@@ -328,6 +405,7 @@ tc_conv_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
     }
     if (p.dbg && blockIdx.x == 0 && threadIdx.x == 128) {
       p.dbg[2] = t_wait; p.dbg[3] = clock64() - t_all; p.dbg[5] = C::STAGES;
+      p.dbg[8] = (long long)p.sk_count; p.dbg[9] = 8 * 2 * kSkMaxGrid;    // the fixup counters (tests)
     }
   }
 }
@@ -376,8 +454,43 @@ int g_pair_px = 1;       // unflow_set_int_option("tc_pair_px"): 1 = narrow tran
 int g_ksplit = 1;        // unflow_set_int_option("tc_ksplit"): 1 = layers with few tiles cut their K loops into slices, 0 = never
 long long *g_dbg = nullptr;   // unflow_tc_conv_debug: device buffer of 16 long longs for the role timers of CTA 0
 
+// Stream-K fixup storage, per device, allocated on first use and kept: 2 partial-sum slots per CTA (its first and
+// its last segment; a range holds at most two pieces of split tiles) of 128 x BN floats at BN = 128, and one
+// counter per SK item (fewer than 2 x grid) and consumer warp, which the last arriver resets to zero.  A launch
+// uses them from start to end, so tc_conv launches on one device must run one at a time: on one stream (as every
+// caller in this project does), never side by side on two.
+static int sk_storage(float **part, unsigned **count) {
+  static float *parts[64] = {};
+  static unsigned *counts[64] = {};
+  int dev = 0;
+  cudaError_t e = cudaGetDevice(&dev);
+  if (e == cudaSuccess && (dev < 0 || dev >= 64)) { set_error("tc_conv: device %d out of range", dev); return UNFLOW_ECUDA; }
+  if (e == cudaSuccess && !parts[dev]) {
+    // may be first reached inside a graph capture: allocate and zero outside it, on a stream of our own
+    cudaStreamCaptureMode mode = cudaStreamCaptureModeRelaxed;
+    cudaThreadExchangeStreamCaptureMode(&mode);
+    float *pp = nullptr;
+    unsigned *cc = nullptr;
+    cudaStream_t s = nullptr;
+    const size_t n_count = 8 * 2 * kSkMaxGrid;
+    e = cudaMalloc(&pp, sizeof(float) * 2 * kSkMaxGrid * BM * 128);
+    if (e == cudaSuccess) e = cudaMalloc(&cc, sizeof(unsigned) * n_count);
+    if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking);
+    if (e == cudaSuccess) e = cudaMemsetAsync(cc, 0, sizeof(unsigned) * n_count, s);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+    if (s) cudaStreamDestroy(s);
+    cudaThreadExchangeStreamCaptureMode(&mode);
+    if (e == cudaSuccess) { parts[dev] = pp; counts[dev] = cc; }
+    else { cudaFree(pp); cudaFree(cc); }
+  }
+  if (e != cudaSuccess) { set_error("tc_conv: stream-K storage: %s", cudaGetErrorString(e)); return UNFLOW_ECUDA; }
+  *part = parts[dev];
+  *count = counts[dev];
+  return UNFLOW_OK;
+}
+
 template <int BN>
-static int launch(const CUtensorMap &mA, const CUtensorMap &mBh, const CUtensorMap &mBl, const ConvParams &p,
+static int launch(const CUtensorMap &mA, const CUtensorMap &mBh, const CUtensorMap &mBl, ConvParams &p,
                   cudaStream_t stream) {
   using C = Cfg<BN>;
   static bool attr_set = false;
@@ -386,9 +499,11 @@ static int launch(const CUtensorMap &mA, const CUtensorMap &mBh, const CUtensorM
     if (e != cudaSuccess) { set_error("tc_conv: cannot opt in to %d bytes of shared memory: %s", C::SMEM_BYTES, cudaGetErrorString(e)); return UNFLOW_ECUDA; }
     attr_set = true;
   }
-  const long long total = (long long)p.n_classes * p.tiles_n * p.tiles_y * p.tiles_x * p.n_blocks * p.ksplit;
-  const int grid = total < kNumSMs ? (int)total : kNumSMs;
-  tc_conv_kernel<BN><<<grid, NTHREADS, C::SMEM_BYTES, stream>>>(mA, mBh, mBl, p);
+  // one CTA per SM: DP waves of whole items, then the last items' K blocks spread over the grid where that pays
+  const int total = p.n_classes * p.tiles_n * p.tiles_y * p.tiles_x * p.n_blocks * p.ksplit;
+  make_sk_schedule(p.sk, total, kNumSMs, p.chunk, [&](int w) { return work_len(p, w); });
+  if (int rc = sk_storage(&p.sk_part, &p.sk_count)) return rc;
+  tc_conv_kernel<BN><<<p.sk.grid, NTHREADS, C::SMEM_BYTES, stream>>>(mA, mBh, mBl, p);
   count_launch();
   return check_launch("tc_conv_kernel");
 }
@@ -406,7 +521,7 @@ inline int choose_ksplit(const ConvParams &p) {
 
 // tile -> kernel: encodes the two weight-plane maps (box = BN rows, or BN / 2 for pair_px) and launches
 static int launch_bn(int BN, const CUtensorMap &mA, const float *w_hi, const float *w_lo, const cuuint64_t *wdims,
-                     const cuuint64_t *wstrides, const ConvParams &p, cudaStream_t stream) {
+                     const cuuint64_t *wstrides, ConvParams &p, cudaStream_t stream) {
   CUtensorMap mBh, mBl;
   cuuint32_t box[3] = {(cuuint32_t)BK, (cuuint32_t)(p.pair_px ? BN / 2 : BN), 1};
   cuuint32_t estr[3] = {1, 1, 1};

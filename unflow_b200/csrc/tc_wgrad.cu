@@ -29,7 +29,8 @@
 // (tap, 32-channel group) pairs, so a layer with few input channels fills the tile with several taps at
 // once (conv2: 64 channels -> two taps per block).  A chunk is a run of 32-pixel K blocks sized so that the
 // grid has a few waves of items; items of one chunk are adjacent in the schedule, so the chunk's
-// activations are read from HBM once and re-read from L2.
+// activations are read from HBM once and re-read from L2.  The last items are cut into K ranges spread evenly
+// over the grid (tc_schedule.h); each range ends in the same red.add epilogue.
 //   warp 0           TMA into the raw ring: per K block 4 boxes of P (32 px x 32 ch each) and BN/32 boxes of G
 //                    (element stride = the conv stride, tap offset in the start coordinate, zero fill outside)
 //   warpgroups 1, 2  each splits + transposes half of the G tile from a raw slot into a split slot; then (after
@@ -67,6 +68,7 @@ struct WgradParams {
   int stride, stride_x, pad_t, pad_l;   // stride_x = 1 in the row-window form (x stride inside the tensor map)
   float *dw;
   long long pitch_r, pitch_t;       // dW[r * pitch_r + t * pitch_t + c]
+  SkSchedule sk;                    // the segments of each CTA (tc_schedule.h): every one ends in red.add
 };
 
 // Two rings.  Raw slot (TMA): [P raw] [G raw], per 32-channel group [32 px][32 ch]; the P boxes in the 128-byte
@@ -105,9 +107,13 @@ __device__ __forceinline__ Item decode_item(const WgradParams &p, int it) {
   w.chunk = it;
   return w;
 }
-__device__ __forceinline__ int chunk_len(const WgradParams &p, int chunk) {
+__device__ __host__ __forceinline__ int chunk_len(const WgradParams &p, int chunk) {
   const int k0 = chunk * p.kc;
   return (k0 + p.kc <= p.n_ptiles) ? p.kc : p.n_ptiles - k0;
+}
+// K blocks of work item `it` (the schedule's item length)
+__device__ __host__ __forceinline__ int item_len(const WgradParams &p, int it) {
+  return chunk_len(p, it / (p.r_blocks * p.c_blocks));
 }
 
 // Fragment sets of the consumer, as in tc_conv.cu: K step k of a K block uses set k % FRAG_SETS and is one wgmma
@@ -149,7 +155,6 @@ tc_wgrad_kernel(const __grid_constant__ CUtensorMap mapP, const __grid_constant_
   auto split_empty = [&](int s) { return bars + 8u * (2 * C::RAW_STAGES + s); };  // MMAs of both on split slot s done
 
   const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0), lane = threadIdx.x & 31;   // warp-uniform: see tc_conv.cu
-  const int total_items = p.n_chunks * p.r_blocks * p.c_blocks;
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < C::RAW_STAGES; ++s) {
@@ -170,8 +175,10 @@ tc_wgrad_kernel(const __grid_constant__ CUtensorMap mapP, const __grid_constant_
     int s = 0;
     unsigned ph = 0;
     long long t_wait = 0, t_all = clock64();
-    for (int item = blockIdx.x; item < total_items; item += gridDim.x) {
-      const Item w = decode_item(p, item);
+    const SegmentWalk walk = segment_walk(p.sk);
+    for (int q = 0; q < walk.n_seg; ++q) {
+      const Segment sg = segment_at(p.sk, walk, q);
+      const Item w = decode_item(p, sg.item);
       int gch[GROUPS], gdx[GROUPS], gdy[GROUPS];           // per column group: channel, tap offset
 #pragma unroll
       for (int j = 0; j < GROUPS; ++j) {
@@ -183,8 +190,8 @@ tc_wgrad_kernel(const __grid_constant__ CUtensorMap mapP, const __grid_constant_
           gch[j] = p.cgroups * 32; gdx[j] = gdy[j] = 0;    // past the last group: channels >= C, TMA zero fill
         }
       }
-      const int k0 = w.chunk * p.kc, klen = chunk_len(p, w.chunk);
-      for (int kb = k0; kb < k0 + klen; ++kb) {
+      const int k0 = w.chunk * p.kc, k1 = sg.k1 < 0 ? chunk_len(p, w.chunk) : sg.k1;
+      for (int kb = k0 + sg.k0; kb < k0 + k1; ++kb) {
         int q = kb;
         const int px = (q % p.tiles_x) * p.TW; q /= p.tiles_x;
         const int py = (q % p.tiles_y) * p.TH; q /= p.tiles_y;
@@ -232,9 +239,12 @@ tc_wgrad_kernel(const __grid_constant__ CUtensorMap mapP, const __grid_constant_
     };
     float sum[R], acc[R];
     unsigned a_hi[FRAG_SETS][4], a_lo[FRAG_SETS][4];
-    for (int item = blockIdx.x; item < total_items; item += gridDim.x) {
-      const Item w = decode_item(p, item);
-      const int iters = chunk_len(p, w.chunk);
+    const SegmentWalk walk = segment_walk(p.sk);
+    for (int q = 0; q < walk.n_seg; ++q) {
+      // a segment starts on a chunk boundary of its item: its chunks are the item's chunks
+      const Segment sg = segment_at(p.sk, walk, q);
+      const Item w = decode_item(p, sg.item);
+      const int iters = (sg.k1 < 0 ? chunk_len(p, w.chunk) : sg.k1) - sg.k0;
       if (w.rb * BM + 64 * cw >= p.R) {
         // all 64 rows of this warpgroup are past R: its half of G only (the other warpgroup reads it)
         for (int it = 0; it < iters; ++it) {
@@ -328,7 +338,7 @@ tc_wgrad_kernel(const __grid_constant__ CUtensorMap mapP, const __grid_constant_
 }
 
 template <int BN>
-static int launch(const CUtensorMap &mP, const CUtensorMap &mG, const WgradParams &p, cudaStream_t stream) {
+static int launch(const CUtensorMap &mP, const CUtensorMap &mG, WgradParams &p, cudaStream_t stream) {
   using C = Cfg<BN>;
   static bool attr_set = false;
   if (!attr_set) {
@@ -336,14 +346,15 @@ static int launch(const CUtensorMap &mP, const CUtensorMap &mG, const WgradParam
     if (e != cudaSuccess) { set_error("tc_wgrad: cannot opt in to %d bytes of shared memory: %s", C::SMEM_BYTES, cudaGetErrorString(e)); return UNFLOW_ECUDA; }
     attr_set = true;
   }
-  const long long total = (long long)p.n_chunks * p.r_blocks * p.c_blocks;
-  const int grid = total < kNumSMs ? (int)total : kNumSMs;
-  tc_wgrad_kernel<BN><<<grid, NTHREADS, C::SMEM_BYTES, stream>>>(mP, mG, p);
+  // one CTA per SM: DP waves of whole items, then the last items' K blocks spread over the grid where that pays
+  make_sk_schedule(p.sk, p.n_chunks * p.r_blocks * p.c_blocks, kNumSMs, p.chunk,
+                   [&](int it) { return item_len(p, it); });
+  tc_wgrad_kernel<BN><<<p.sk.grid, NTHREADS, C::SMEM_BYTES, stream>>>(mP, mG, p);
   count_launch();
   return check_launch("tc_wgrad_kernel");
 }
 
-static int launch_bn(int BN, const CUtensorMap &mP, const CUtensorMap &mG, const WgradParams &p, cudaStream_t stream) {
+static int launch_bn(int BN, const CUtensorMap &mP, const CUtensorMap &mG, WgradParams &p, cudaStream_t stream) {
   if (BN == 128) return launch<128>(mP, mG, p, stream);
   if (BN == 64) return launch<64>(mP, mG, p, stream);
   return launch<32>(mP, mG, p, stream);
