@@ -200,7 +200,9 @@ def main(argv=None):
                     help='; '.join('%s: %s' % (d, ', '.join(v)) for d, (v, _) in DATASETS.items()))
     ap.add_argument('--ex', default='', help='Experiment name(s) (can be comma separated list).')
     ap.add_argument('--num', type=int, default=10, help='Number of examples to evaluate. -1 = all.')
-    ap.add_argument('--gpu', default='0')
+    ap.add_argument('--gpu', default='0',
+                    help='GPU id(s), comma separated; evaluation runs on the first listed id (eval_gui.py '
+                         'sets CUDA_VISIBLE_DEVICES to the list and uses its first device)')
     ap.add_argument('--output_benchmark', action='store_true', help='Output raw flow files.')
     ap.add_argument('--output_visual', action='store_true', help='Output flow visualization files.')
     ap.add_argument('--output_backward', action='store_true', help='Output backward flow files.')

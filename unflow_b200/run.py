@@ -2,11 +2,18 @@
 (/root/reference/src/run.py:21-33, src/e2eflow/util.py:37-62, src/e2eflow/core/train.py:116-145):
 
     python -m unflow_b200.run --ex NAME [--debug] [--ow] [--config PATH] [--synthetic]
-    python -m torch.distributed.run --nproc-per-node N -m unflow_b200.run --ex NAME   (data parallel)
+    python -m torch.distributed.run --nproc-per-node N -m unflow_b200.run --ex NAME   (alternative launcher)
 
 * ``config.ini`` sections [dirs] [run] [train] [train_<dataset>] are parsed with the same type
   coercion (int -> float -> bool -> str); the dataset section overrides [train]
   (run.py:91-92); ``manual_decay_*`` strings become lists and define ``num_iters``.
+* [run] gpu_list (run.py:40-49, ``launch.py``): ``gpu_list = 3`` trains in this process on GPU 3;
+  ``gpu_list = 0,1,2,3`` trains data parallel from the one command above -- it starts one worker per
+  listed GPU (worker k on the k-th listed GPU, ``CUDA_VISIBLE_DEVICES`` set to the list), waits on them and
+  stops them all when one fails or the command is interrupted.  Ids count the devices the command sees;
+  duplicate, negative or absent ids are rejected before anything starts.  Without the key the run trains
+  on ``cuda:LOCAL_RANK``; under an external launcher (``WORLD_SIZE`` set) gpu_list is not used and the
+  launcher's processes train.
 * [run] batch_size is the TOTAL batch, divided by the number of GPUs (run.py:48).
 * training runs in chunks of ``save_interval`` iterations; after each chunk a checkpoint is
   written and training resumes from the newest checkpoint by parsing the iteration from the file
@@ -55,6 +62,7 @@ import copy
 import glob
 import os
 import shutil
+import sys
 
 import torch
 import torch.distributed as dist
@@ -365,6 +373,16 @@ def main(argv=None):
     local = int(os.environ.get('LOCAL_RANK', '0'))
     if not torch.cuda.is_available():
         raise SystemExit("unflow_b200.run needs a CUDA device (no CPU fallback)")
+    from . import launch
+    gpu_ids = launch.resolve(run_config, torch.cuda.device_count())
+    if gpu_ids is not None and len(gpu_ids) > 1:
+        # the workers do all the work, rank 0 the experiment directories; this process creates no CUDA context
+        code = launch.launch(sys.argv[1:] if argv is None else argv, gpu_ids)
+        if code:
+            raise SystemExit(code)
+        return
+    if gpu_ids is not None:
+        local = gpu_ids[0]
     torch.cuda.set_device(local)
     device = torch.device('cuda', local)
     if world > 1:
@@ -470,7 +488,6 @@ def main(argv=None):
         if args.graph:
             # ncclCommDestroy was observed to hang for minutes when the communicator had been used
             # inside a captured CUDA graph (bench.py:_finish): leave once every rank is done
-            import sys
             torch.cuda.synchronize()
             dist.barrier()
             sys.stdout.flush()
