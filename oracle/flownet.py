@@ -13,6 +13,11 @@ Variables are passed explicitly as a dict  TF-variable-name -> tensor in TF
 layout (conv ``weights``: [kh,kw,in,out]; conv2d_transpose ``weights``:
 [kh,kw,out,in]; ``biases``: [out]) -- the checkpoint contract of the
 reference (train.py:23-65, scopes flownet.py:30-75).
+
+The graph runs in the dtype and on the device of its inputs (the variables are cast to them), so the
+same restatement serves as a float64 GPU reference.  The two custom ops it calls are the module
+attributes ``correlation`` and ``image_warp``: the CPU float32 ops by default, replaceable by ops of
+another precision (tests/test_gpu_float64_network.py), as is the activation ``leaky_relu``.
 """
 import torch
 
@@ -23,8 +28,23 @@ from .image_warp import image_warp
 FLOW_SCALE = 5.0  # flownet.py:11
 
 
+def correlation(in0, in1):
+    """The FlowNetC cost volume with the reference's attributes (flownet.py:209-211)."""
+    return _ops.correlation(in0, in1, pad=20, kernel_size=1, max_displacement=20, stride_1=1, stride_2=2)
+
+
 def _leaky_relu(x):  # flownet.py:84-86
     return torch.maximum(0.1 * x, x)
+
+
+def leaky_relu(x, scope):
+    """The activation of layer ``scope``; replaceable (e.g. by one that takes its side of the kink from another
+    run of the network)."""
+    return _leaky_relu(x)
+
+
+def _var(t, like):
+    return torch.as_tensor(t).to(dtype=like.dtype, device=like.device)
 
 
 class _Scope:
@@ -36,16 +56,16 @@ class _Scope:
         return _Scope(self.v, self.p + name + '/')
 
     def conv(self, x, name, stride=1, act=True):
-        w = torch.as_tensor(self.v[self.p + name + '/weights']).float().permute(3, 2, 0, 1).contiguous()
-        b = torch.as_tensor(self.v[self.p + name + '/biases']).float()
+        w = _var(self.v[self.p + name + '/weights'], x).permute(3, 2, 0, 1).contiguous()
+        b = _var(self.v[self.p + name + '/biases'], x)
         y = tfc.conv2d_same(x, w, b, stride)
-        return _leaky_relu(y) if act else y
+        return leaky_relu(y, self.p + name) if act else y
 
     def deconv(self, x, name, act=True):
-        w = torch.as_tensor(self.v[self.p + name + '/weights']).float().permute(3, 2, 0, 1).contiguous()
-        b = torch.as_tensor(self.v[self.p + name + '/biases']).float()
+        w = _var(self.v[self.p + name + '/weights'], x).permute(3, 2, 0, 1).contiguous()
+        b = _var(self.v[self.p + name + '/biases'], x)
         y = tfc.conv2d_transpose_same(x, w, b, 2)
-        return _leaky_relu(y) if act else y
+        return leaky_relu(y, self.p + name) if act else y
 
 
 def _flownet_upconv(s, conv6_1, conv5_1, conv4_1, conv3_1, conv2, conv1=None, inputs=None,
@@ -115,8 +135,7 @@ def flownet_c_features(s, im):  # flownet.py:195-206
 
 
 def flownet_c(s, conv3_a, conv3_b, conv2_a, full_res=False):  # flownet.py:209-237
-    corr = _ops.correlation(conv3_a, conv3_b, pad=20, kernel_size=1, max_displacement=20,
-                            stride_1=1, stride_2=2)
+    corr = correlation(conv3_a, conv3_b)
     conv_redir = s.conv(conv3_a, 'conv_redir')
     conv3_1 = s.conv(torch.cat([conv_redir, corr], 1), 'conv3_1')
     conv4 = s.conv(conv3_1, 'conv4', 2)

@@ -17,8 +17,8 @@ from .unsupervised import regularization_loss
 
 
 def supervised_loss(variables, batch, params, normalization=None, photometric_draws=None):
-    mean = torch.tensor(normalization[0], dtype=torch.float32) / 255.0        # :13
     im1, im2, flow_gt, mask_gt = batch                                         # :14
+    mean = torch.tensor(normalization[0], dtype=torch.float32, device=im1.device) / 255.0     # :13
     im1, im2 = im1 / 255.0, im2 / 255.0                                        # :15-16
     im_shape = im1.shape[1:3]
     if photometric_draws is not None:                                          # :21-26

@@ -48,19 +48,21 @@ def conv2d_transpose_same(x, w, b, stride=2):
 
 
 def resize_bilinear_legacy(x, size):
-    """x: [B,H,W,C] -> [B,size[0],size[1],C]; TF1 align_corners=False."""
+    """x: [B,H,W,C] -> [B,size[0],size[1],C]; TF1 align_corners=False.  The ratios, source positions and
+    fractions are float32 as in TF's kernel; the interpolation runs in x's dtype, on x's device."""
     B, H, W, C = x.shape
     oh, ow = int(size[0]), int(size[1])
-    hs = torch.tensor(H / oh, dtype=torch.float32)
-    ws = torch.tensor(W / ow, dtype=torch.float32)
-    iy = torch.arange(oh, dtype=torch.float32) * hs
-    ix = torch.arange(ow, dtype=torch.float32) * ws
+    dev = x.device
+    hs = torch.tensor(H / oh, dtype=torch.float32, device=dev)
+    ws = torch.tensor(W / ow, dtype=torch.float32, device=dev)
+    iy = torch.arange(oh, dtype=torch.float32, device=dev) * hs
+    ix = torch.arange(ow, dtype=torch.float32, device=dev) * ws
     y0 = iy.floor().long()
     y1 = torch.clamp(iy.ceil().long(), max=H - 1)
     x0 = ix.floor().long()
     x1 = torch.clamp(ix.ceil().long(), max=W - 1)
-    ly = (iy - y0.float()).view(1, oh, 1, 1)
-    lx = (ix - x0.float()).view(1, 1, ow, 1)
+    ly = (iy - y0.float()).view(1, oh, 1, 1).to(x.dtype)
+    lx = (ix - x0.float()).view(1, 1, ow, 1).to(x.dtype)
     top_rows = x[:, y0]
     bot_rows = x[:, y1]
     tl, tr = top_rows[:, :, x0], top_rows[:, :, x1]

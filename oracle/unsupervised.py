@@ -20,11 +20,11 @@ LOSSES = ['occ', 'sym', 'fb', 'grad', 'ternary', 'photo', 'smooth_1st', 'smooth_
 
 def regularization_loss(variables, scale=0.0004):
     """slim.l2_regularizer(0.0004) on every conv / deconv ``weights`` variable
-    (flownet.py:176,200,218): scale * sum(w^2) / 2, summed over variables."""
-    total = torch.zeros(())
-    for name, v in variables.items():
-        if name.endswith('/weights'):
-            total = total + scale * (torch.sum(torch.as_tensor(v).float() ** 2) / 2)
+    (flownet.py:176,200,218): scale * sum(w^2) / 2, summed over variables, in their dtype."""
+    ws = [torch.as_tensor(v) for name, v in variables.items() if name.endswith('/weights')]
+    total = torch.zeros((), dtype=ws[0].dtype, device=ws[0].device) if ws else torch.zeros(())
+    for w in ws:
+        total = total + scale * (torch.sum(w ** 2) / 2)
     return total
 
 
