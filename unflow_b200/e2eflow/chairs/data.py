@@ -26,15 +26,19 @@ class ChairsData(Data):
 
     def _check(self):
         self._require('flying_chairs')
-        local_path = os.path.join(self.current_dir, 'flying_chairs')
-        release = (os.path.isdir(os.path.join(local_path, 'FlyingChairs_release', 'data'))
-                   and os.path.isfile(os.path.join(local_path, 'FlyingChairs_train_val.txt')))
-        if release and not os.path.isfile(os.path.join(local_path, CONVERTED_MARKER)):
-            convert_release(local_path)
+        convert_if_release(os.path.join(self.current_dir, 'flying_chairs'))
         self._require(*(os.path.join('flying_chairs', d) for d in OUTPUT_DIRS))
 
     def get_raw_dirs(self):
         return [os.path.join(self.current_dir, 'flying_chairs', 'image')]
+
+
+def convert_if_release(local_path):
+    """``convert_release`` when ``local_path`` holds the release layout and no finished conversion."""
+    release = (os.path.isdir(os.path.join(local_path, 'FlyingChairs_release', 'data'))
+               and os.path.isfile(os.path.join(local_path, 'FlyingChairs_train_val.txt')))
+    if release and not os.path.isfile(os.path.join(local_path, CONVERTED_MARKER)):
+        convert_release(local_path)
 
 
 def convert_release(local_path):

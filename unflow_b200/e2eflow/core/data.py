@@ -2,9 +2,32 @@
 
 The reference's ``Data`` downloads and unpacks a dataset whose directory is missing; here nothing is
 ever fetched: a missing directory is a ``FileNotFoundError`` naming the layout the adapter expects.
-``fast_dir``, when given, is read instead of ``data_dir`` (the reference copies the dataset there
-first; here it must already be in place)."""
+``fast_dir``, when given, is read instead of ``data_dir``.  As the reference's ``Data.__init__``
+(core/data.py:27-36) does, ``run`` first copies the adapter's ``dirs`` from ``data_dir`` into
+``fast_dir`` where they are missing there (``stage``); staged copies are never removed."""
 import os
+import shutil
+
+
+def stage(data_dir, fast_dir, dirs):
+    """Copy every entry of ``dirs`` that is a directory under ``data_dir`` and missing under ``fast_dir``.
+    A copy is made in ``<dst>.partial`` and renamed to ``<dst>`` once complete, so an interrupted copy
+    is never taken for a dataset: the next call discards it and copies again.  Directories already
+    under ``fast_dir`` are not touched.  Returns the entries copied."""
+    copied = []
+    for d in dirs:
+        src, dst = os.path.join(data_dir, d), os.path.join(fast_dir, d)
+        if os.path.isdir(dst) or not os.path.isdir(src):
+            continue
+        partial = dst + '.partial'
+        if os.path.isdir(partial):
+            shutil.rmtree(partial)
+        print(">> Copying {} to {}".format(d, fast_dir))
+        shutil.copytree(src, partial)
+        os.rename(partial, dst)
+        print(">> Copied {}".format(d))
+        copied.append(d)
+    return copied
 
 
 class Data():

@@ -23,6 +23,19 @@
   core/tf_checkpoint.py), which the reference's Saver can restore.  Either kind is accepted on
   resume and for ``finetune``.  ``--ow`` discards an existing experiment, ``--debug`` disables
   checkpoint writing.
+* experiment directories (experiment.py): when training ends -- also when there was nothing left to
+  train ("max_iter reached") -- rank 0 concludes the experiment (run.py:204-205): the newest checkpoint
+  of [dirs] checkpoints /<name> is copied into [dirs] log /ex/<name>, the directory meant to be backed
+  up, next to the earlier concluded ones; not with ``--debug``.  At start-up, when [dirs] checkpoints
+  /<name> holds no checkpoint (missing or emptied) and log/ex/<name> does -- a concluded run or a
+  pretrained model extracted there -- that one is copied back and training continues from it, with the
+  reference's "Warning: intermediate checkpoints could not be restored."  Copies go through a temporary
+  name and a rename, so a half-copied checkpoint is never visible under its final name.  ``--ow`` also
+  removes the concluded checkpoints.
+* [dirs] fast: before reading a dataset, local rank 0 of each node copies the KITTI directories and
+  those of the training dataset from [dirs] data into [dirs] fast where they are missing there (a
+  FlyingChairs release is converted in [dirs] data first), while the other ranks wait; the run then
+  reads [dirs] fast.  An interrupted copy is redone by the next run; staged copies are kept.
 * ``finetune = exA,exB`` ([train*] sections): network i of the stack is initialised from the
   newest checkpoint of experiment i -- looked up in [dirs] checkpoints, then [dirs] log /ex --
   with the reference's rules (util.py:75-85, train.py:23-62): when the experiment has no
@@ -59,6 +72,8 @@
 import argparse
 import configparser
 import copy
+import datetime
+import filecmp
 import glob
 import os
 import shutil
@@ -69,6 +84,7 @@ import torch.distributed as dist
 
 KITTI_NORMALIZATION = ([104.920005, 110.1753, 114.785955], 1 / 0.0039216)  # core/input.py:45-46
 FT_HOLD_OUT = 40    # pairs of each KITTI training set kept out of the fine-tune for evaluation (run.py:187-188)
+STAGING_TIMEOUT = datetime.timedelta(hours=24)     # how long ranks wait for [dirs] fast to be filled
 
 
 def config_dict(config_path):
@@ -192,6 +208,95 @@ def save_checkpoint(trainer, ckpt_dir, iteration, fmt='pt'):
     return prefix + '.pt'
 
 
+def _replace_atomically(dst, write):
+    """``write(tmp)`` fills ``dst + '.partial'``, which is flushed to disk and renamed to ``dst``; the
+    directory is flushed after the rename, so the new name also survives a power loss.  Under its final
+    name a file is complete or absent.  A failed write leaves no temporary file behind."""
+    tmp = dst + '.partial'
+    try:
+        write(tmp)
+        with open(tmp, 'rb+') as f:
+            os.fsync(f.fileno())
+        os.replace(tmp, dst)
+    except BaseException:
+        if os.path.exists(tmp):
+            os.remove(tmp)
+        raise
+    fd = os.open(os.path.dirname(os.path.abspath(dst)), os.O_RDONLY)
+    try:
+        os.fsync(fd)
+    finally:
+        os.close(fd)
+
+
+def _write_text(path, text):
+    with open(path, 'w') as f:
+        f.write(text)
+
+
+def copy_checkpoint(path, dst_dir):
+    """experiment.py:61-74 (``_copy_latest_checkpoint``): the checkpoint ``path`` -- a ``.pt`` file or a TF
+    prefix, as ``latest_checkpoint`` returns it -- copied into ``dst_dir`` under its own name.  A TF
+    checkpoint's ``.data`` and ``.index`` files are followed by a ``checkpoint`` state file naming only
+    this checkpoint, as the reference writes it.  Every file is replaced atomically and the state file
+    comes last, so ``latest_checkpoint(dst_dir)`` finds the previous newest checkpoint or this complete
+    one, never a part of it.  Files already there with the same bytes are left alone (a run concluded
+    again).  A different TF checkpoint of the same name loses its ``.index`` before its ``.data`` is
+    replaced, so no reader pairs the new data with the old index.  Returns the copy's path (or prefix)."""
+    os.makedirs(dst_dir, exist_ok=True)
+    src_dir, base = os.path.split(path)
+    names = [base] if path.endswith('.pt') else [base + '.data-00000-of-00001', base + '.index']
+    pending = [n for n in names if not (os.path.isfile(os.path.join(dst_dir, n)) and
+                                        filecmp.cmp(os.path.join(src_dir, n), os.path.join(dst_dir, n),
+                                                    shallow=False))]
+    index = os.path.join(dst_dir, base + '.index')
+    if not path.endswith('.pt') and pending and os.path.isfile(index):
+        os.remove(index)
+        pending = [n for n in names if n in pending or n.endswith('.index')]
+    for name in pending:
+        _replace_atomically(os.path.join(dst_dir, name),
+                            lambda tmp, name=name: shutil.copyfile(os.path.join(src_dir, name), tmp))
+    if not path.endswith('.pt'):
+        state = 'model_checkpoint_path: "%s"\nall_model_checkpoint_paths: "%s"\n' % (base, base)
+        _replace_atomically(os.path.join(dst_dir, 'checkpoint'), lambda tmp: _write_text(tmp, state))
+    return os.path.join(dst_dir, base)
+
+
+def conclude(ckpt_dir, ex_dir):
+    """experiment.py:79-83 (``Experiment.conclude``): the newest checkpoint of ``ckpt_dir`` ([dirs]
+    checkpoints /<name>, which need not be kept) copied into ``ex_dir`` ([dirs] log /ex/<name>, which
+    should be backed up).  Earlier concluded checkpoints stay.  Returns the copy's path, or None when
+    ``ckpt_dir`` holds no checkpoint."""
+    ck = latest_checkpoint(ckpt_dir)
+    if ck is None:
+        print('Warning: no checkpoints written')
+        return None
+    return copy_checkpoint(ck[1], ex_dir)
+
+
+def restore_concluded(ckpt_dir, ex_dir):
+    """experiment.py:36-45 (``Experiment.__init__``): when ``ckpt_dir`` holds no checkpoint (missing or
+    emptied) but ``ex_dir`` does -- a concluded experiment, or a pretrained model extracted there -- the
+    newest one of ``ex_dir`` is copied into ``ckpt_dir``, so training continues from it.  Returns the
+    copy's path, or None when nothing was copied."""
+    if latest_checkpoint(ckpt_dir) is not None:
+        return None
+    ck = latest_checkpoint(ex_dir)
+    if ck is None:
+        return None
+    path = copy_checkpoint(ck[1], ckpt_dir)
+    print('Warning: intermediate checkpoints could not be restored.')
+    return path
+
+
+def remove_concluded(ex_dir):
+    """``--ow``: the concluded checkpoints of ``ex_dir`` (``model.ckpt-*`` and the ``checkpoint`` state
+    file) removed, so that a fresh run does not later restore the discarded model."""
+    for p in glob.glob(os.path.join(ex_dir, 'model.ckpt-*')) + [os.path.join(ex_dir, 'checkpoint')]:
+        if os.path.isfile(p):
+            os.remove(p)
+
+
 def kitti_inputs(dirs, run_config, params, train_dataset, gpu_batch_size, start_iter, rank, world):
     """The 'kitti' branch of the reference run.py (:31-58, :96-115): training batches from the raw
     sequences (``input_raw(swap_images=False, center_crop=True, shift=iterations_done * batch_size)``)
@@ -270,6 +375,32 @@ def dataset_inputs(dirs, run_config, params, train_dataset, gpu_batch_size, star
     if os.path.isdir(os.path.join(kdata.current_dir, 'data_stereo_flow', 'training', 'flow_occ')):
         eval_input = KITTIInput(data=kdata, batch_size=1, normalize=False, dims=(384, 1280))
     return batches, eval_input
+
+
+def stage_datasets(data_dir, fast_dir, train_dataset, local_rank=0):
+    """[dirs] fast (core/data.py:27-36, run.py:53-56): the directories of the KITTI adapter, which the
+    reference builds with ``fast_dir`` whatever it trains on, and of ``train_dataset``'s adapter, copied
+    from ``data_dir`` into ``fast_dir`` where they are missing there (``data.stage``).  A FlyingChairs
+    release is converted in ``data_dir`` first, so the converted tree is what is copied.  Only local
+    rank 0 copies (the node's ranks share its disk); on other ranks this does nothing.  Returns the
+    directories copied."""
+    if local_rank != 0:
+        return []
+    from .e2eflow.core.data import stage
+    from .e2eflow.kitti.data import KITTIData
+    dirs = list(KITTIData.dirs)
+    if train_dataset == 'chairs':
+        from .e2eflow.chairs.data import ChairsData, convert_if_release
+        if not os.path.isdir(os.path.join(fast_dir, 'flying_chairs')):
+            convert_if_release(os.path.join(data_dir, 'flying_chairs'))
+        dirs += ChairsData.dirs
+    elif train_dataset == 'synthia':
+        from .e2eflow.synthia.data import SynthiaData
+        dirs += SynthiaData.dirs
+    elif train_dataset == 'cityscapes':
+        from .e2eflow.cityscapes.data import CityscapesData
+        dirs += CityscapesData.dirs
+    return stage(data_dir, fast_dir, dirs)
 
 
 def evaluate_kitti(trainer, eval_input, device, hold_out_inv=None, dataset='2012', loss_averages=None):
@@ -370,7 +501,7 @@ def main(argv=None):
 
     world = int(os.environ.get('WORLD_SIZE', '1'))
     rank = int(os.environ.get('RANK', '0'))
-    local = int(os.environ.get('LOCAL_RANK', '0'))
+    local_rank = int(os.environ.get('LOCAL_RANK', '0'))
     if not torch.cuda.is_available():
         raise SystemExit("unflow_b200.run needs a CUDA device (no CPU fallback)")
     from . import launch
@@ -381,8 +512,7 @@ def main(argv=None):
         if code:
             raise SystemExit(code)
         return
-    if gpu_ids is not None:
-        local = gpu_ids[0]
+    local = gpu_ids[0] if gpu_ids is not None else local_rank
     torch.cuda.set_device(local)
     device = torch.device('cuda', local)
     if world > 1:
@@ -392,14 +522,18 @@ def main(argv=None):
 
     log_dir = dirs.get('log', '../log')
     ckpt_dir = os.path.join(dirs.get('checkpoints', os.path.join(log_dir, 'checkpoints')), args.ex)
+    ex_dir = os.path.join(log_dir, 'ex', args.ex)
     if rank == 0:
-        if args.ow and os.path.isdir(ckpt_dir):
-            shutil.rmtree(ckpt_dir)
+        if args.ow:
+            if os.path.isdir(ckpt_dir):
+                shutil.rmtree(ckpt_dir)
+            remove_concluded(ex_dir)
         os.makedirs(ckpt_dir, exist_ok=True)
+        # before the barrier below: every rank's latest_checkpoint then finds the restored checkpoint
+        restore_concluded(ckpt_dir, ex_dir)
         # experiment.py (Experiment.__init__): the run's config is kept in log/ex/<name>/config.ini -- where
         # eval.py (eval_gui.py:97-116) looks for the parameters a checkpoint was trained with
         if not args.debug and os.path.isfile(args.config):
-            ex_dir = os.path.join(log_dir, 'ex', args.ex)
             os.makedirs(ex_dir, exist_ok=True)
             if args.ow or not os.path.isfile(os.path.join(ex_dir, 'config.ini')):
                 shutil.copyfile(args.config, os.path.join(ex_dir, 'config.ini'))
@@ -435,6 +569,8 @@ def main(argv=None):
         restore_checkpoint(tr, source[1], nets=[i])
     if start_iter > num_iters:
         print('-- train: max_iter reached')
+        if rank == 0 and not args.debug:      # run.py:204-205 concludes after tr.run however it returned
+            conclude(ckpt_dir, ex_dir)
         for w in (train_writer, eval_writer):
             if w is not None:
                 w.close()
@@ -446,6 +582,13 @@ def main(argv=None):
     batches, eval_input = None, None
     data_dir = dirs.get('data', '')
     if not args.synthetic and os.path.isdir(data_dir):
+        if dirs.get('fast'):
+            # copying a dataset can outlast NCCL's collective timeout: the ranks wait for the copies on a gloo
+            # group that allows for it
+            group = dist.new_group(backend='gloo', timeout=STAGING_TIMEOUT) if world > 1 else None
+            stage_datasets(data_dir, dirs['fast'], train_dataset, local_rank)
+            if group is not None:
+                dist.barrier(group=group)
         batches, eval_input = dataset_inputs(dirs, run_config, params, train_dataset, gpu_batch_size,
                                              start_iter, rank, world)
     for i in range(start_iter, num_iters + 1):
@@ -481,6 +624,8 @@ def main(argv=None):
                 dist.barrier()
     if batches is not None:
         batches.close()
+    if rank == 0 and not args.debug:      # after the last chunk's barrier; the other ranks need not wait
+        conclude(ckpt_dir, ex_dir)
     for w in (train_writer, eval_writer):
         if w is not None:
             w.close()
