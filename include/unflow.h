@@ -311,7 +311,10 @@ int unflow_conv3x3_narrow_wgrad(const float *x, long long x_pitch, const float *
  *           (slim.conv2d_transpose and the input gradient of mode 0; Hout, Wout % stride == 0)
  *   stride 1 or 2, kh*kw <= 64.  UNFLOW_EINVAL otherwise.
  *   Epilogue: y = act(bias + conv), or with accumulate != 0  y += act(bias + conv) (the activation applies
- *   to this call's sum only, never to what y held before); bias may be null, act = 0 skips the activation. */
+ *   to this call's sum only, never to what y held before); bias may be null, act = 0 skips the activation.
+ *   Cin <= 4 (the flow heads' input gradients, the flow up-sampling deconvs) runs in exact fp32 on the FMA pipes
+ *   instead (csrc/conv_fma.cu): one launch, each output element written by one thread, channels >= Cout never;
+ *   the weight planes are read as hi + lo. */
 /* Debug hook: CTA 0 of every following tc_conv launch writes its role timers
  * (clocks blocked on each pipeline barrier / in total, see csrc/tc_conv.cu) into `buf`, device memory for 16
  * long longs; nullptr switches it off.  [0, 1]: producer wait / total, [2, 3]: consumer wait / total; tc_conv

@@ -20,6 +20,11 @@ operands still alive, replayed alone with the same pointers and shapes:
   * role timers of CTA 0 (unflow_tc_conv_debug) from one more launch: the stages of the ring, the fraction of
     its cycles the producer waits for a free stage (raw slot), and the consumers wait for a loaded one (and,
     for wgrad, for a free split slot).
+  * path (conv): wgmma, or fma for the contractions over at most 4 channels that unflow_tc_conv runs on the FMA
+    pipes (csrc/conv_fma.cu).  Those rows have no plan, schedule or role timers; they show the bytes the launch
+    must move (the input once, the output written, and read too when the launch accumulates), the achieved
+    GB/s and that amount's time at the data-sheet HBM3 bandwidth (3.35 TB/s, H100 SXM), with one total line.
+  * wgrad: one more line with the launches of R = 2 rows (the weight gradients of the flow up-sampling deconvs).
   * --compare-lib PATH: the destination of this launch computed with this library twice and with the library
     at PATH twice, from the same start and on the same operands: whether the two libraries agree bit for bit,
     and the largest difference between them against the largest between two runs of the other library
@@ -49,6 +54,8 @@ from float64_refs import view  # noqa: E402
 from unflow_b200 import synthetic as synth  # noqa: E402
 
 TF32_TFLOPS = 989.0 / 2          # H100 SXM data sheet, dense: bf16 / 2
+HBM_GBS = 3350.0                 # H100 SXM data sheet, HBM3
+FMA_MAX_CIN = 4                  # csrc/tc_conv.cu: unflow_tc_conv runs contractions over <= 4 channels in conv_fma.cu
 GRID = 132                       # CTAs of a tc launch (one per SM)
 CHUNK = 8                        # K blocks per accumulation chunk (tc_chunk default): the stream-K cut unit
 
@@ -146,7 +153,10 @@ def geometry(lib, name, a):
         pix = N * (Hin * Win if mode == 1 else Hout * Wout)
         row = dict(kind="deconv" if mode == 1 else "conv", acc=bool(accumulate), taps="%d/%d" % (kh * kw, stride),
                    shape="%dx%dx%dx%d>%dx%dx%d" % (N, Hin, Win, Cin, Hout, Wout, Cout),
-                   BN=BN, ksplit=ks, items=tiles * ncls * nblk * ks)
+                   BN=BN, ksplit=ks, items=tiles * ncls * nblk * ks, path="wgmma")
+        if Cin <= FMA_MAX_CIN:
+            row.update(path="fma", bytes=4 * (N * Hin * Win * Cin + N * Hout * Wout * Cout * (2 if accumulate else 1)))
+            return y, (N * Hout * Wout - 1) * y_pitch + Cout, 2 * pix * Cout * Cin * kh * kw, row, False
         row["dp"], row["sk"], row["sk_segments"] = schedule(conv_lengths(tiles, ncls, nblk, ks, class_k))
         return y, (N * Hout * Wout - 1) * y_pitch + Cout, 2 * pix * Cout * Cin * kh * kw, row, ks > 1
     if name == "unflow_tc_conv_window":
@@ -155,7 +165,7 @@ def geometry(lib, name, a):
                                                             pad_t, 0))
         row = dict(kind="window", acc=False, taps="%d/%d" % (kh, stride),
                    shape="%dx%dx%dx%d>%dx%dx%d" % (N, H, Wout, 8 * Cp, Hout, Wout, Cout),
-                   BN=BN, ksplit=1, items=tiles * ncls * nblk)
+                   BN=BN, ksplit=1, items=tiles * ncls * nblk, path="wgmma")
         row["dp"], row["sk"], row["sk_segments"] = schedule(conv_lengths(tiles, ncls, nblk, 1, class_k))
         return y, (N * Hout * Wout - 1) * y_pitch + Cout, 2 * N * Hout * Wout * Cout * 8 * Cp * kh, row, False
     if name == "unflow_tc_wgrad":
@@ -168,7 +178,7 @@ def geometry(lib, name, a):
         n_dw, flops, kind, taps = R * kh * 8 * Cp, 2 * N * Ho * Wo * R * 8 * Cp * kh, "window", kh
     v = (ctypes.c_int * 15)()
     assert lib.unflow_tc_wgrad_plan(*plan, v) == 15
-    row = dict(kind=kind, taps="%d/%d" % (taps, stride), shape="%dx%dx%d, %dx%d" % (plan[:5]),
+    row = dict(kind=kind, taps="%d/%d" % (taps, stride), shape="%dx%dx%d, %dx%d" % (plan[:5]), R=R,
                BN=v[11], kc=v[7], n_chunks=v[8], items=v[8] * v[9] * v[10])
     row["dp"], row["sk"], row["sk_segments"] = schedule(
         [min(v[7], v[6] - c * v[7]) for c in range(v[8]) for _ in range(v[9] * v[10])])
@@ -237,11 +247,12 @@ class Bench:
                 times.append(e0.elapsed_time(e1) * 1e3 / self.args.reps)
             del g
             dbg = torch.zeros(16, dtype=torch.int64, device="cuda")
-            self._real.unflow_tc_conv_debug(dbg.data_ptr())
-            try:
-                self.launch(self._real, name, a, s)
-            finally:
-                self._real.unflow_tc_conv_debug(None)
+            if row.get("path") != "fma":           # the FMA kernel has no role timers
+                self._real.unflow_tc_conv_debug(dbg.data_ptr())
+                try:
+                    self.launch(self._real, name, a, s)
+                finally:
+                    self._real.unflow_tc_conv_debug(None)
             torch.cuda.synchronize()
             t = dbg.tolist()
             cmp = None
@@ -256,6 +267,8 @@ class Bench:
                    tf32_share=3 * flops / (us * 1e-6) / 1e12 / TF32_TFLOPS,
                    cons_full_wait=t[2] / max(t[3], 1), prod_empty_wait=t[0] / max(t[1], 1),
                    cons_split_wait=(t[4] / max(t[3], 1)) if wgrad and t[5] else None, sliced=sliced, compare=cmp)
+        if row.get("path") == "fma":
+            row.update(gbs=row["bytes"] / (us * 1e-6) / 1e9, floor_us=row["bytes"] / (HBM_GBS * 1e9) * 1e6)
         self.rows.append(row)
         print(fmt(self.args.kernel, len(self.rows) - 1, row), flush=True)
 
@@ -276,9 +289,9 @@ class Bench:
 
 
 HEAD = {
-    "conv": "%3s %-6s %-3s %-26s %-6s %4s %3s %5s %6s %5s %5s %5s %6s %8s %6s %6s %6s" % (
-        "#", "kind", "acc", "N x Hin x Win x Cin>out", "taps/s", "BN", "ks", "items", "waves", "DP", "SK", "segs",
-        "stages", "us", "tf32", "c.full", "p.empt"),
+    "conv": "%3s %-5s %-6s %-3s %-26s %-6s %4s %3s %5s %6s %5s %5s %5s %6s %8s %6s %6s %6s" % (
+        "#", "path", "kind", "acc", "N x Hin x Win x Cin>out", "taps/s", "BN", "ks", "items", "waves", "DP", "SK",
+        "segs", "stages", "us", "tf32", "c.full", "p.empt"),
     "wgrad": "%3s %-6s %-22s %-7s %4s %3s %3s %5s %6s %5s %5s %5s %6s %8s %6s %6s %6s %6s" % (
         "#", "kind", "N x Hp x Wp, R x C", "taps/s", "BN", "kc", "ch", "items", "waves", "DP", "SK", "segs",
         "stages", "us", "tf32", "c.full", "p.empt", "c.splt"),
@@ -287,9 +300,15 @@ HEAD = {
 
 def fmt(kernel, i, r):
     st = "+".join("%d" % x for x in r["stages"]) if r["stages"] else "-"
-    if kernel == "conv":
-        line = "%3d %-6s %-3s %-26s %-6s %4d %3d %5d %6.2f %5d %5d %5d %6s %8.1f %5.1f%% %5.1f%% %5.1f%%" % (
-            i, r["kind"], "+=" if r["acc"] else "", r["shape"], r["taps"], r["BN"], r["ksplit"], r["items"],
+    if kernel == "conv" and r["path"] == "fma":
+        # no plan, schedule or role timers: the bytes the launch must move, the rate it moved them at, their time
+        # at the data-sheet HBM bandwidth
+        line = "%3d %-5s %-6s %-3s %-26s %-6s %46s %8.1f  %.1f MB, %.0f GB/s, HBM floor %.1f us" % (
+            i, "fma", r["kind"], "+=" if r["acc"] else "", r["shape"], r["taps"], "", r["us"], r["bytes"] / 1e6,
+            r["gbs"], r["floor_us"])
+    elif kernel == "conv":
+        line = "%3d %-5s %-6s %-3s %-26s %-6s %4d %3d %5d %6.2f %5d %5d %5d %6s %8.1f %5.1f%% %5.1f%% %5.1f%%" % (
+            i, r["path"], r["kind"], "+=" if r["acc"] else "", r["shape"], r["taps"], r["BN"], r["ksplit"], r["items"],
             r["items"] / GRID, r["dp"], r["sk"], r["sk_segments"], st, r["us"], 100 * r["tf32_share"], 100 * r["cons_full_wait"], 100 * r["prod_empty_wait"])
     else:
         line = "%3d %-6s %-22s %-7s %4d %3d %3d %5d %6.2f %5d %5d %5d %6s %8.1f %5.1f%% %5.1f%% %5.1f%% %6s" % (
@@ -359,6 +378,15 @@ def main():
           "throttle reasons %s" % (len(proxy.rows), total / 1e3, info.get("name"), info.get("power.limit"),
                                    clocks["sm_mhz"], info.get("clocks.max.sm"), clocks["samples"],
                                    clocks["reasons"]))
+    fma = [r for r in proxy.rows if r.get("path") == "fma"]
+    if fma:
+        print("fma: %d launches, %.1f us in all, %.1f MB at %.0f GB/s (HBM floor %.1f us)" % (
+            len(fma), sum(r["us"] for r in fma), sum(r["bytes"] for r in fma) / 1e6,
+            sum(r["bytes"] for r in fma) / (sum(r["us"] for r in fma) * 1e-6) / 1e9, sum(r["floor_us"] for r in fma)))
+    r2 = [(i, r) for i, r in enumerate(proxy.rows) if r.get("R") == 2]
+    if r2:
+        print("R = 2: %d launches, %.1f us in all (%s)" % (
+            len(r2), sum(r["us"] for _, r in r2), ", ".join("#%d %.1f us" % (i, r["us"]) for i, r in r2)))
     if other is not None:
         single = [r for r in proxy.rows if not r["sliced"]]
         print("compare: %d/%d launches with one part along K bit-identical; worst max|new-old| / max|old-old| on "

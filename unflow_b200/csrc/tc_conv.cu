@@ -50,45 +50,12 @@
 // (round to nearest) bounds it.
 #include <algorithm>
 
-#include "tc_common.cuh"
+#include "tc_conv_plan.cuh"
 
 namespace unflow {
 namespace tc {
 
-constexpr int MAX_TAPS = 64;
 constexpr int NTHREADS = 384;    // warpgroup 0: TMA producer (warp 0); warpgroups 1-2: consumers
-
-struct Tap {
-  short dx, dy;
-  int widx;
-  int widx2;                  // pair_px: the weight tap of the px = 1 class for this input offset (-1: none)
-};
-
-struct ConvParams {
-  int N, Hit, Wit;            // images; iteration rows / columns of one class
-  int TW, TH, TN;             // tile box, TW*TH*TN <= 128
-  int tiles_x, tiles_y, tiles_n, n_blocks, n_classes;
-  int s_in_x, s_in_y, s_out;    // input strides per axis (the row-window form folds the x stride into the tensor map)
-  int Cin, Cout, kblocks;
-  float *out;
-  long long out_pitch;        // floats between consecutive output pixels
-  int Hout, Wout;
-  const float *bias;          // [Cout] or nullptr
-  float slope;                // leaky-ReLU slope when act != 0
-  int act, accumulate;
-  int chunk;                  // K blocks per wgmma accumulation between two register adds (g_chunk)
-  long long *dbg;             // role timers of CTA 0 (unflow_tc_conv_debug), or nullptr
-  int pair_px;                // two output-parity classes (px = 0, 1) of a narrow transposed layer share one tile, see
-                              // pair_px_plan()
-  int ksplit;                 // > 1: the K loop of a tile is cut into ksplit work items whose partial sums meet in the
-                              // (zeroed) output through red.global.add; bias / activation run as a separate pass
-  int class_start[5];
-  short class_px[4], class_py[4];
-  Tap taps[MAX_TAPS];
-  SkSchedule sk;              // the segments of each CTA (tc_schedule.h)
-  float *sk_part;             // stream-K fixup: partial sums of split tiles, 2 slots per CTA (see sk_storage)
-  unsigned *sk_count;         // stream-K fixup: arrivals per SK item and consumer warp, zero between launches
-};
 
 // Stage: [A raw fp32] [B hi] [B lo].  Each 1024-byte aligned (128-byte swizzle atoms).  The ring fills the opt-in
 // limit: BN = 128: 4 x 48 KB, BN = 64: 7 x 32 KB, BN = 32: 8 x 24 KB (capped at 8).
@@ -707,9 +674,13 @@ extern "C" int unflow_tc_conv(const float *x, int N, int Hin, int Win, int Cin, 
   int BN = 0;
   int rc0 = make_plan(p, BN, N, Hin, Win, Cin, Hout, Wout, Cout, mode, stride, kh, kw, pad_t, pad_l);
   if (rc0) return rc0;
-  pair_px_plan(p, BN, mode, stride, Cout);
   p.out = y; p.out_pitch = y_pitch;
   p.bias = bias; p.slope = slope; p.act = act; p.accumulate = accumulate;
+  // A contraction over at most 4 channels fills one 32-channel K block per tap with 28 zero channels: with 3 MMA
+  // passes its useful rate is at most 495 / 3 * 4 / 32 ~ 21 TFLOP/s, below the FMA pipes' 67, and both paths write
+  // the same bytes.  Such layers (the flow heads' input gradients, the flow up-sampling deconvs) run in conv_fma.cu.
+  if (Cin <= 4) return tc::conv_fma(p, x, Hin, Win, x_pitch, w_hi, w_lo, (cudaStream_t)stream);
+  pair_px_plan(p, BN, mode, stride, Cout);
   // K slices (few tiles, long K): partial sums are added into the output, which is zeroed first unless the call
   // accumulates anyway; bias + leaky ReLU then run as unflow_bias_lrelu over the (dense) result.  That pass sees
   // only the sum in y, so a call that accumulates into y and needs it (y += act(bias + conv)) is not sliced.

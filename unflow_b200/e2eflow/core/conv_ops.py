@@ -380,6 +380,8 @@ class _DeconvTC(torch.autograd.Function):
 # fill the GPU with 16x32-pixel tiles, the coarse ones (flow4 .. flow6: 8 .. 48 tiles) split the input
 # channels over several CTAs per tile (csrc/narrow_conv.cu, csplit).  On the tensor-core kernel a head is
 # one 32-wide N block with 2 useful columns and a K of 9 x 1026 walked by a handful of CTAs: 0.5 ms per step.
+# The input gradient (a contraction over the 2 flow channels) goes through tc_conv.run, which unflow_tc_conv
+# runs on the FMA pipes like every contraction over at most 4 channels (csrc/conv_fma.cu).
 def _use_narrow(x, w, stride, pads):
     from . import tc_conv
     return (w.shape[0] == 2 and w.shape[2] == 3 and w.shape[3] == 3 and stride in (1, (1, 1))
@@ -389,8 +391,9 @@ def _use_narrow(x, w, stride, pads):
 
 class _NarrowConv3x3(torch.autograd.Function):
     """The 2-channel flow heads (csrc/narrow_conv.cu): forward and weight gradient in exact fp32 on
-    the FMA pipes, reading the wide input once at any pixel pitch; the input gradient (C_in wide) runs
-    on the tensor-core kernel."""
+    the FMA pipes, reading the wide input once at any pixel pitch; the input gradient (C_in wide, a
+    contraction over the 2 flow channels) goes through ``tc_conv.run`` and runs on the FMA pipes too
+    (csrc/conv_fma.cu)."""
 
     @staticmethod
     def forward(ctx, x, w, b):
