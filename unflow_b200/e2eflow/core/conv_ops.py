@@ -2,14 +2,19 @@
 
 'fp32'    plain cuDNN float32 (what the reference's slim.conv2d computes, flownet.py:174-233);
           no tensor cores.
-'3xtf32'  the same contraction on the tensor cores at fp32-level accuracy (the default of bench.py and the
-          trainer): every operand is split x = hi + lo (hi = TF32-rounded, lo = exact residual) and
-          lo*hi' + hi*lo' + hi*hi' is accumulated by the hand-written wgmma kernels (csrc/tc_conv.cu: forward
-          and input gradient, csrc/tc_wgrad.cu: weight gradient, csrc/narrow_conv*.cu: the 2-channel flow
+'3xtf32'  the same contraction on the tensor cores at fp32-level accuracy (the default of bench.py; run.py
+          and eval.py use it with ``[run] conv_precision = 3xtf32``): every operand is split x = hi + lo
+          (hi = TF32-rounded, lo = exact residual) and lo*hi' + hi*lo' + hi*hi' is accumulated by the
+          hand-written wgmma kernels (csrc/tc_conv.cu: forward and input gradient, csrc/tc_wgrad.cu: weight
+          gradient, csrc/narrow_conv*.cu: the 2-channel flow
           heads in exact fp32) with the K loop cut into chunks that are summed in fp32 registers: 1.8e-6 of
           max|y| against float64 per layer, and the same 1e-4 flow tolerance against the fp32 oracle as the
           plain fp32 path.  Every layer runs on these kernels; an input they cannot read in place is copied
           into a fresh NHWC buffer first (_tc_input).
+
+The mode is process-global.  Importing core/flownet.py sets it from ``UNFLOW_CONV_PRECISION`` (default
+'fp32'); run.py then applies ``[run] conv_precision`` when the config has it, and eval.py the key of each
+experiment's copied config.
 """
 import torch
 import torch.nn.functional as F

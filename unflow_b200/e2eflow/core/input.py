@@ -14,17 +14,18 @@ Python and is what decides WHICH frames are trained on.  That logic is kept verb
 * ``_input_images`` (:78-107): sorted files, (2i, 2i+1) are a pair; ``hold_out_inv`` keeps the first
   k pairs of a ``random.seed(0)`` shuffle.
 
-Instead of TF queues a batch iterator with a small prefetch thread decodes PNGs (OpenCV) into
-pinned host tensors ``[B,H,W,3]`` float32 in [0,255], RGB like ``tf.image.decode_png``; with
-``num_threads`` > 1 the pairs of a batch are decoded on a pool of that many threads, into the same
-slots with the same crop seeds (bit-identical batches).
+Instead of TF queues ``DecodeAhead`` decodes PNGs (OpenCV) into pinned host tensors ``[B,H,W,3]``
+float32 in [0,255], RGB like ``tf.image.decode_png``, a few batches ahead of the training loop: every
+frame is one task on a pool of ``num_threads`` threads, and tasks of consecutive batches run together,
+so up to ``num_threads`` decodes are in flight whatever the batch size.  Each pair lands in its own
+slot with the crop seed drawn for it in order, so the batches are bit-identical for any thread count.
 * ``sequence_pairs`` / ``sequence_files`` (sintel/input.py, middlebury/input.py): per sorted
   sequence directory frame k paired with frame k + 1, and the sorted per-sequence ground-truth lists.
 With ``rank`` / ``world_size`` each rank takes every world_size-th batch: distinct shards per GPU
 (the reference's towers all dequeue the same batch, SURVEY.md R4).
 """
+import collections
 import os
-import queue
 import random
 import threading
 
@@ -91,49 +92,121 @@ def resize_output_flow(t, height, width, channels=2):
     return impl(t, height, width, channels)
 
 
-class _Prefetcher:
-    """Iterator over ``make(i)`` for i = first, first+step, ... produced by a daemon thread."""
+class _PendingBatch:
+    """One batch of a ``DecodeAhead`` stream while its reads run: each item's ``finish`` runs on the
+    thread that completes the item's last read, and ``done`` is set once every item has finished or
+    any read or finish has failed (``error``)."""
 
-    def __init__(self, make, first, step, depth=4, pool=None):
-        self._q = queue.Queue(maxsize=depth)
-        self._stop = threading.Event()
-        self._pool = pool
+    def __init__(self, out, items):
+        self.out = out
+        self.items = items
+        self.decoded = [[None] * len(reads) for reads, _ in items]
+        self.left = [len(reads) for reads, _ in items]
+        self.unfinished = len(items)
+        self.error = None
+        self.lock = threading.Lock()
+        self.done = threading.Event()
 
-        def work():
-            i = first
-            while not self._stop.is_set():
-                try:
-                    item = make(i)
-                except BaseException as e:   # surfaced in the consumer
-                    item = e
-                while not self._stop.is_set():
-                    try:
-                        self._q.put(item, timeout=0.1)
-                        break
-                    except queue.Full:
-                        continue
-                if isinstance(item, BaseException):
-                    return
-                i += step
+    def run(self, k, j):
+        """Read j of item k; the item's finish when it was the last one outstanding."""
+        try:
+            if self.done.is_set():          # an earlier task of this batch failed: nothing more to do
+                return
+            self.decoded[k][j] = self.items[k][0][j]()
+            with self.lock:
+                self.left[k] -= 1
+                last = self.left[k] == 0
+            if not last:
+                return
+            self.items[k][1](*self.decoded[k])
+            self.decoded[k] = None
+            with self.lock:
+                self.unfinished -= 1
+                if self.unfinished == 0:
+                    self.done.set()
+        except BaseException as e:      # surfaced in the consumer
+            with self.lock:
+                if self.error is None:
+                    self.error = e
+            self.done.set()
 
-        self._t = threading.Thread(target=work, daemon=True)
-        self._t.start()
+
+class DecodeAhead:
+    """Iterator over the batches ``first, first + step, first + 2 step, ...`` of a stream, decoded ahead
+    on a pool of ``num_threads`` threads ([run] num_input_threads; OpenCV releases the GIL).
+
+    ``plan(i)`` describes batch i as ``(out, items)``: ``out`` is what the iterator yields for it and
+    every item is ``(reads, finish)``.  Each ``read()`` is one task on the pool (one file decode), and
+    ``finish(*results)`` runs once all reads of its item are done, on the thread that did the last one;
+    it writes that item's slot of ``out`` and nothing else, so the batch does not depend on which thread
+    ran what.  ``plan`` runs on the consumer's thread, in batch order, so anything it draws (crop seeds)
+    is drawn in the same order for any thread count.  Pinned host memory is therefore allocated, and
+    released, on the consumer's thread only: the pool threads make no CUDA call, which would invalidate a
+    CUDA graph the training loop may be capturing at that moment (``run.py --graph``).
+
+    The reads of ``depth`` batches are queued ahead of the batch the consumer holds, in stream order:
+    enough that ``num_threads`` decodes stay in flight across batch boundaries (at least 4 batches, as
+    many as ``num_threads`` reads need), and no more, so memory stays at ``depth`` + 2 batches.
+    ``__next__`` plans the next batch before it takes one, so a failing ``plan`` raises there and leaves
+    the stream as it was: no decoded batch is lost and a later call plans it again.  A failed read or
+    finish is raised by ``__next__`` for its batch, and the stream stays failed.  ``close()`` cancels the
+    queued reads and waits for the running ones (one decode each), so no pool thread is left behind; a
+    constructor that fails does the same before it raises."""
+
+    def __init__(self, plan, first, step, num_threads):
+        from concurrent.futures import ThreadPoolExecutor
+        self._plan = plan
+        self._next_index = first
+        self._step = step
+        self._pool = ThreadPoolExecutor(max(num_threads, 1), thread_name_prefix='decode')
+        self._pending = collections.deque()
+        self._error = None
+        try:
+            reads = self._submit()
+            self.depth = max(4, -(-max(num_threads, 1) // max(reads, 1)))
+            self._top_up()
+        except BaseException:
+            self.close()
+            raise
+
+    def _submit(self):
+        """Plans the next batch of the stream and queues its reads; returns how many."""
+        out, items = self._plan(self._next_index)
+        self._next_index += self._step
+        batch = _PendingBatch(out, items)
+        self._pending.append(batch)
+        n = 0
+        for k, (reads, _) in enumerate(items):
+            for j in range(len(reads)):
+                self._pool.submit(batch.run, k, j)
+                n += 1
+        return n
+
+    def _top_up(self):
+        """The batch ``__next__`` returns next and ``depth`` batches behind it queued."""
+        while len(self._pending) <= self.depth:
+            self._submit()
 
     def __iter__(self):
         return self
 
     def __next__(self):
-        item = self._q.get()
-        if isinstance(item, StopIteration):
-            raise StopIteration
-        if isinstance(item, BaseException):
-            raise item
-        return item
+        if self._error is not None:
+            raise self._error
+        self._top_up()
+        batch = self._pending[0]
+        batch.done.wait()
+        if batch.error is not None:
+            self._error = batch.error
+            self.close()
+            raise batch.error
+        self._pending.popleft()
+        out, batch.out, batch.items = batch.out, None, None    # the pool keeps no reference to the batch
+        return out
 
     def close(self):
-        self._stop.set()
-        if self._pool is not None:
-            self._pool.shutdown(wait=False)
+        self._pool.shutdown(wait=True, cancel_futures=True)
+        self._pending.clear()
 
 
 class Input():
@@ -163,24 +236,6 @@ class Input():
         if self.normalize:
             image = self._normalize_image(image)
         return image
-
-    def _decode_pool(self):
-        """A pool of ``num_threads`` decode threads ([run] num_input_threads; OpenCV releases the GIL),
-        None for one thread."""
-        if self.num_threads <= 1:
-            return None
-        from concurrent.futures import ThreadPoolExecutor
-        return ThreadPoolExecutor(self.num_threads, thread_name_prefix='decode')
-
-    @staticmethod
-    def _fill(pool, load, n):
-        """``load(k)`` for k < n: in order on the calling thread, or spread over ``pool``.  Each
-        ``load`` writes only its own slot k of the batch, so both give the same batch."""
-        if pool is None:
-            for k in range(n):
-                load(k)
-        else:
-            list(pool.map(load, range(n)))
 
     # -- which files ---------------------------------------------------------------------------
     def raw_pairs(self, swap_images=True, sequence=True, shift=0, seed=0, skip=0):
@@ -273,9 +328,7 @@ class Input():
         B = self.batch_size
         pin = torch.cuda.is_available() if pin is None else pin
 
-        pool = self._decode_pool()
-
-        def make(batch_index):
+        def plan(batch_index):
             gen = torch.Generator().manual_seed(crop_seed * 1000003 + batch_index)
             # the crop seeds of the whole batch are drawn first, in order, so they do not depend on
             # which thread decodes which pair
@@ -283,22 +336,24 @@ class Input():
             a = torch.empty((B, height, width, 3), dtype=torch.float32, pin_memory=pin)
             b = torch.empty((B, height, width, 3), dtype=torch.float32, pin_memory=pin)
 
-            def load(k):
+            def item(k):
                 fn1, fn2 = pairs[(batch_index * B + k) % len(pairs)]
-                im1, im2 = read_png_image(fn1), read_png_image(fn2)
-                if needs_crop:
-                    im1, im2 = augment.random_crop([im1, im2], [height, width, 3], seed=seeds[k])
-                else:
-                    im1, im2 = im1.reshape(height, width, 3), im2.reshape(height, width, 3)
-                if self.normalize:
-                    im1, im2 = self._normalize_image(im1), self._normalize_image(im2)
-                a[k].copy_(im1)
-                b[k].copy_(im2)
 
-            self._fill(pool, load, B)
-            return a, b
+                def finish(im1, im2):
+                    if needs_crop:
+                        im1, im2 = augment.random_crop([im1, im2], [height, width, 3], seed=seeds[k])
+                    else:
+                        im1, im2 = im1.reshape(height, width, 3), im2.reshape(height, width, 3)
+                    if self.normalize:
+                        im1, im2 = self._normalize_image(im1), self._normalize_image(im2)
+                    a[k].copy_(im1)
+                    b[k].copy_(im2)
+                # the two frames are separate decode tasks
+                return (lambda: read_png_image(fn1), lambda: read_png_image(fn2)), finish
 
-        return _Prefetcher(make, rank, world_size, pool=pool)
+            return (a, b), [item(k) for k in range(B)]
+
+        return DecodeAhead(plan, rank, world_size, self.num_threads)
 
     def _input_test(self, image_dir, hold_out_inv=None):
         """One pass over the pairs of ``image_dir``: ``(im1, im2, input_shape)`` with batch 1

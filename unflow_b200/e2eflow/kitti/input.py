@@ -8,7 +8,7 @@ import torch
 
 from ..core import augment
 from ..core.flow_io import read_kitti_flow
-from ..core.input import Input, _Prefetcher, read_png_image, resize_image_with_crop_or_pad
+from ..core.input import DecodeAhead, Input, read_png_image, resize_image_with_crop_or_pad
 
 # (image directory, ground-truth directory) of the two training sets input_train_gt draws from
 TRAIN_GT_SETS = [('data_scene_flow/training/image_2', 'data_scene_flow/training/flow_occ'),
@@ -101,25 +101,26 @@ class KITTIInput(Input):
         B = self.batch_size
         pin = torch.cuda.is_available() if pin is None else pin
 
-        pool = self._decode_pool()
+        def read_gt(path):
+            flow, mask = read_kitti_flow(path)
+            return torch.cat([torch.as_tensor(flow), torch.as_tensor(mask)], 2).float()
 
-        def make(batch_index):
+        def plan(batch_index):
             gen = torch.Generator().manual_seed(crop_seed * 1000003 + batch_index)
             seeds = [int(torch.randint(0, 2 ** 31 - 1, (1,), generator=gen)) for _ in range(B)]
             out = [torch.empty((B, height, width, c), dtype=torch.float32, pin_memory=pin) for c in (3, 3, 2, 1)]
 
-            def load(k):
+            def item(k):
                 fn1, fn2, fn_gt = triples[(batch_index * B + k) % len(triples)]
-                im1, im2 = read_png_image(fn1), read_png_image(fn2)
-                flow, mask = read_kitti_flow(fn_gt)
-                gt = torch.cat([torch.as_tensor(flow), torch.as_tensor(mask)], 2).float()
-                im1, im2, gt = augment.random_crop([im1, im2, gt], [height, width, 3], seed=seeds[k])
-                if self.normalize:
-                    im1, im2 = self._normalize_image(im1), self._normalize_image(im2)
-                for dst, src in zip(out, (im1, im2, gt[:, :, 0:2], gt[:, :, 2:3])):
-                    dst[k].copy_(src)
 
-            self._fill(pool, load, B)
-            return tuple(out)
+                def finish(im1, im2, gt):
+                    im1, im2, gt = augment.random_crop([im1, im2, gt], [height, width, 3], seed=seeds[k])
+                    if self.normalize:
+                        im1, im2 = self._normalize_image(im1), self._normalize_image(im2)
+                    for dst, src in zip(out, (im1, im2, gt[:, :, 0:2], gt[:, :, 2:3])):
+                        dst[k].copy_(src)
+                return (lambda: read_png_image(fn1), lambda: read_png_image(fn2), lambda: read_gt(fn_gt)), finish
 
-        return _Prefetcher(make, rank, world_size, pool=pool)
+            return tuple(out), [item(k) for k in range(B)]
+
+        return DecodeAhead(plan, rank, world_size, self.num_threads)

@@ -9,7 +9,9 @@ Datasets and variants: kitti (train_2012, train_2015, test_2012, test_2015), cha
 sintel (train_clean, train_final, test_clean, test_final), mdb (train, test); with ``--num -1``
 the Sintel test variants evaluate 552 pairs and Middlebury test 12, as the reference does.
 
-For every experiment in ``--ex`` the newest checkpoint is looked up under [dirs] log /ex/<name>, then
+For every experiment in ``--ex`` the conv arithmetic is set from ``[run] conv_precision`` of the config
+copied into its experiment directory (``fp32`` | ``3xtf32``; without the key the process's mode, from
+``UNFLOW_CONV_PRECISION``, else fp32), and the newest checkpoint is looked up under [dirs] log /ex/<name>, then
 [dirs] checkpoints/<name> (eval_gui.py:100-108; TensorFlow checkpoints of the reference and this
 implementation's ``.pt`` files are both accepted), the networks are restored, and every example is
 run at the dataset's fixed size (KITTI 384x1280, FlyingChairs 384x512, Sintel 512x1024,
@@ -30,7 +32,7 @@ import sys
 import numpy as np
 import torch
 
-from .run import config_dict, convert_input_strings, latest_checkpoint
+from .run import config_dict, conv_precision, convert_input_strings, latest_checkpoint
 
 KITTI_VARIANTS = ('train_2012', 'train_2015', 'test_2012', 'test_2015')
 # dataset -> (variants, network input height x width) (eval_gui.py:298-322)
@@ -172,8 +174,10 @@ def evaluate_examples(name, items, dims, flow_fn, device, num=10, out_dir=None, 
     return averages
 
 
-def experiment_setup(name, default_config_path, dataset):
-    """eval_gui.py:97-116: experiment directory, its config and its newest checkpoint."""
+def experiment_setup(name, default_config_path, dataset, conv_default=None):
+    """eval_gui.py:97-116: experiment directory, its config and its newest checkpoint.  Sets the conv
+    arithmetic to the config's [run] conv_precision, so that an experiment is evaluated in the mode it was
+    trained in; without the key to ``conv_default`` (None: the current mode)."""
     current = config_dict(default_config_path)
     exp_dir = os.path.join(current['dirs'].get('log', ''), 'ex', name)
     config_path = os.path.join(exp_dir, 'config.ini')
@@ -186,6 +190,8 @@ def experiment_setup(name, default_config_path, dataset):
     if ckpt is None:
         raise RuntimeError("Error: experiment must contain a checkpoint")
     config = config_dict(config_path)
+    from .e2eflow.core import conv_ops, flownet
+    flownet.set_conv_precision(conv_precision(config.get('run', {}), conv_default or conv_ops.get_mode()))
     params = config['train']
     convert_input_strings(params, current['dirs'])
     if 'train_' + dataset in config:
@@ -224,8 +230,10 @@ def run_eval(args, device, make_flow_fn=network_flow_fn):
     estimator (the tests substitute a stub to exercise everything around the network on the CPU)."""
     print("-- evaluating: on {} pairs from {}/{}".format(args.num, args.dataset, args.variant))
 
+    from .e2eflow.core import conv_ops
     from .e2eflow.core.flownet import FlowNetVariables
     from .run import restore_checkpoint
+    conv_default = conv_ops.get_mode()      # for experiments whose config does not set [run] conv_precision
     dirs = config_dict(args.config)['dirs']
     data_input, input_fn = dataset_input(args.dataset, args.variant, dirs['data'])
     num = args.num
@@ -233,7 +241,8 @@ def run_eval(args, device, make_flow_fn=network_flow_fn):
         num = ALL_PAIRS.get((args.dataset, args.variant), num)
     results = {}
     for name in [n for n in args.ex.split(',') if n]:
-        params, ckpt, config_path = experiment_setup(name, args.config, args.dataset)
+        params, ckpt, config_path = experiment_setup(name, args.config, args.dataset, conv_default)
+        print("-- evaluating '{}' in conv precision {}".format(name, conv_ops.get_mode()))
         variables = FlowNetVariables(params.get('flownet', 'S'), params.get('full_res'), seed=0).to(device)
 
         class _Holder:       # restore_checkpoint only touches .variables unless optimiser state is asked for

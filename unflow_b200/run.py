@@ -58,9 +58,15 @@
   sequences (consecutive frames, random crop) or the Cityscapes sequences (frame distances 1 and 2,
   random crop) with the reference's arguments (run.py:62-173, ``dataset_inputs``), and like
   ``kitti`` evaluates on the KITTI 2012 training set after every chunk when it is under [dirs] data.
-  [run] num_input_threads threads decode the pairs of a batch (bit-identical batches for any count).
+  [run] num_input_threads threads decode frames a few batches ahead (bit-identical batches for any count).
   With ``--synthetic`` every dataset trains on seeded synthetic pairs of its height x width.
   Datasets are never downloaded: a missing directory is an error naming the expected layout.
+* [run] conv_precision = fp32 | 3xtf32: the arithmetic of the conv / deconv layers (core/conv_ops.py),
+  set before the first network is built, for training and the in-training evaluation.  ``3xtf32`` runs
+  them on the project's wgmma tensor-core kernels, ``fp32`` on cuDNN float32 (the reference's
+  arithmetic).  Without the key the environment variable ``UNFLOW_CONV_PRECISION`` decides, else fp32.
+  Workers started for ``gpu_list`` read the same config, so every rank uses the same mode, and
+  ``eval.py`` evaluates an experiment in the mode of its copied config.
 * TensorBoard summaries (train.py:66-86,187-261,314-370; experiment.py:14-25), from rank 0 only, also
   with ``--debug``: ``<[dirs] log>/ex/<name>/train`` gets the learning rate, every tracked loss and the
   weights of the weighted terms at i = 1 and every ``display_interval`` steps (the steps the loss is
@@ -85,6 +91,7 @@ import torch.distributed as dist
 KITTI_NORMALIZATION = ([104.920005, 110.1753, 114.785955], 1 / 0.0039216)  # core/input.py:45-46
 FT_HOLD_OUT = 40    # pairs of each KITTI training set kept out of the fine-tune for evaluation (run.py:187-188)
 STAGING_TIMEOUT = datetime.timedelta(hours=24)     # how long ranks wait for [dirs] fast to be filled
+CONV_PRECISIONS = ('fp32', '3xtf32')                # core/conv_ops.py
 
 
 def config_dict(config_path):
@@ -132,6 +139,18 @@ def convert_input_strings(config_dct, dirs=None):
             assert ckpt, "Could not load experiment " + name
             found.append(ckpt)
         config_dct['finetune'] = found
+
+
+def conv_precision(run_config, default):
+    """The conv arithmetic ``[run] conv_precision`` asks for: ``fp32`` (cuDNN float32, the reference's
+    arithmetic) or ``3xtf32`` (the wgmma tensor-core kernels at fp32-level accuracy); ``default`` when
+    the key is absent.  Any other value ends the command (SystemExit) naming both."""
+    if 'conv_precision' not in run_config:
+        return default
+    value = run_config['conv_precision']
+    if value not in CONV_PRECISIONS:
+        raise SystemExit('[run] conv_precision = %s: must be %s' % (value, ' or '.join(CONV_PRECISIONS)))
+    return value
 
 
 def latest_checkpoint(ckpt_dir):
@@ -347,7 +366,7 @@ def dataset_inputs(dirs, run_config, params, train_dataset, gpu_batch_size, star
       random-crops, and the pairs that span two snippets of a city directory are kept, as there.
 
     ``shift`` is the reference's resume shift (iterations done x [run] batch_size); each rank reads its
-    own shard of the batch stream; [run] num_input_threads threads decode a batch."""
+    own shard of the batch stream; [run] num_input_threads threads decode ahead of it."""
     if train_dataset in ('kitti', 'kitti_ft'):
         return kitti_inputs(dirs, run_config, params, train_dataset, gpu_batch_size, start_iter, rank, world)
     from .e2eflow.kitti.input import KITTIInput
@@ -494,6 +513,9 @@ def main(argv=None):
 
     cfg = config_dict(args.config)
     dirs, run_config = cfg.get('dirs', {}), cfg['run']
+    # before any network exists; importing flownet first applies UNFLOW_CONV_PRECISION, which the key overrides
+    from .e2eflow.core import conv_ops, flownet
+    precision = flownet.set_conv_precision(conv_precision(run_config, conv_ops.get_mode()))
     train_dataset = run_config.get('dataset', 'kitti')
     params = copy.deepcopy(cfg['train'])
     params.update(cfg.get('train_' + train_dataset, {}))
@@ -578,6 +600,7 @@ def main(argv=None):
     tr.broadcast_variables(0)
     if rank == 0:
         print('-- training from i = {} to {}'.format(start_iter, num_iters))
+    print('-- rank {}: conv precision {}'.format(rank, precision))
 
     batches, eval_input = None, None
     data_dir = dirs.get('data', '')
@@ -591,39 +614,43 @@ def main(argv=None):
                 dist.barrier(group=group)
         batches, eval_input = dataset_inputs(dirs, run_config, params, train_dataset, gpu_batch_size,
                                              start_iter, rank, world)
-    for i in range(start_iter, num_iters + 1):
-        if batches is None:
-            batch = synthetic_batch(gpu_batch_size, params['height'], params['width'], i, rank, device,
-                                    supervised=supervised)
-        else:
-            batch = tuple(t.to(device, non_blocking=True) for t in next(batches))
-        if args.graph and tr._graph is None:
-            tr.capture(*batch)       # leaves parameters, moments and the iteration counter untouched
-        loss = tr.step(*batch)       # LR schedule inside (train.py:225-244)
-        if rank == 0 and (i == 1 or i % params['display_interval'] == 0):
-            print("-- train: i = {}, loss = {}".format(i, float(loss)))
-            write_train_summaries(train_writer, tr, i, learning_rate_at(i - 1, params), images=tr.track_images)
-        if i % save_interval == 0:
-            if not args.debug and rank == 0:
-                save_checkpoint(tr, ckpt_dir, i, args.ckpt_format)
-            if eval_input is not None and rank == 0:      # Trainer.run: self.eval(1) after every chunk
-                loss_averages = {}
-                if supervised:      # the 2015 pairs input_train_gt held out
-                    result = evaluate_kitti(tr, eval_input, device, FT_HOLD_OUT, dataset='2015',
-                                            loss_averages=loss_averages)
-                else:
-                    result = evaluate_kitti(tr, eval_input, device, params.get('eval_hold_out_inv'),
-                                            loss_averages=loss_averages)
-                print("-- eval: i = {}".format(i))
-                for k in sorted(result):
-                    print("   {} = {}".format(k, result[k]))
-                write_eval_summaries(eval_writer, i, result, loss_averages)
-            if world > 1:
-                # rank 0 alone writes the checkpoint and evaluates: the others wait here instead of inside the
-                # next step's all-reduce (where the wait would run into the NCCL watchdog and count as step time)
-                dist.barrier()
-    if batches is not None:
-        batches.close()
+    # the decode pool is stopped however the loop ends (an error, Ctrl-C): its queued reads are cancelled
+    try:
+        for i in range(start_iter, num_iters + 1):
+            if batches is None:
+                batch = synthetic_batch(gpu_batch_size, params['height'], params['width'], i, rank, device,
+                                        supervised=supervised)
+            else:
+                batch = tuple(t.to(device, non_blocking=True) for t in next(batches))
+            if args.graph and tr._graph is None:
+                tr.capture(*batch)       # leaves parameters, moments and the iteration counter untouched
+            loss = tr.step(*batch)       # LR schedule inside (train.py:225-244)
+            if rank == 0 and (i == 1 or i % params['display_interval'] == 0):
+                print("-- train: i = {}, loss = {}".format(i, float(loss)))
+                write_train_summaries(train_writer, tr, i, learning_rate_at(i - 1, params),
+                                      images=tr.track_images)
+            if i % save_interval == 0:
+                if not args.debug and rank == 0:
+                    save_checkpoint(tr, ckpt_dir, i, args.ckpt_format)
+                if eval_input is not None and rank == 0:      # Trainer.run: self.eval(1) after every chunk
+                    loss_averages = {}
+                    if supervised:      # the 2015 pairs input_train_gt held out
+                        result = evaluate_kitti(tr, eval_input, device, FT_HOLD_OUT, dataset='2015',
+                                                loss_averages=loss_averages)
+                    else:
+                        result = evaluate_kitti(tr, eval_input, device, params.get('eval_hold_out_inv'),
+                                                loss_averages=loss_averages)
+                    print("-- eval: i = {}".format(i))
+                    for k in sorted(result):
+                        print("   {} = {}".format(k, result[k]))
+                    write_eval_summaries(eval_writer, i, result, loss_averages)
+                if world > 1:
+                    # rank 0 alone writes the checkpoint and evaluates: the others wait here instead of inside the
+                    # next step's all-reduce (where the wait would run into the NCCL watchdog and count as step time)
+                    dist.barrier()
+    finally:
+        if batches is not None:
+            batches.close()
     if rank == 0 and not args.debug:      # after the last chunk's barrier; the other ranks need not wait
         conclude(ckpt_dir, ex_dir)
     for w in (train_writer, eval_writer):
