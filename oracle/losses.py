@@ -234,7 +234,7 @@ def create_mask(tensor, paddings):  # losses.py:325-335
     inner = torch.ones(max(inner_h, 0), max(inner_w, 0))
     mask2d = torch.nn.functional.pad(inner, (paddings[1][0], paddings[1][1],
                                              paddings[0][0], paddings[0][1]))
-    return mask2d.view(1, H, W, 1).repeat(B, 1, 1, 1)
+    return mask2d.view(1, H, W, 1).repeat(B, 1, 1, 1).to(tensor.device)
 
 
 def create_border_mask(tensor, border_ratio=0.1):  # losses.py:338-344

@@ -108,6 +108,6 @@ def rgb_to_grayscale(x):
 def conv2d_same_nhwc(x, w_hwio):
     """tf.nn.conv2d(x, w, [1,1,1,1], 'SAME') for NHWC x and HWIO weights (odd k)."""
     k = w_hwio.shape[0]
-    w = w_hwio.permute(3, 2, 0, 1).contiguous()
+    w = w_hwio.permute(3, 2, 0, 1).contiguous().to(x)      # (constant filters: in x's dtype, on x's device)
     y = F.conv2d(x.permute(0, 3, 1, 2), w, None, stride=1, padding=k // 2)
     return y.permute(0, 2, 3, 1)

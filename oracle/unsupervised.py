@@ -40,7 +40,7 @@ def unsupervised_loss(variables, batch, params, normalization=None, augment=Fals
                       return_flow=False, return_terms=False):
     if augment:
         raise NotImplementedError("the oracle restates the augment=False graph only")
-    mean = torch.tensor(normalization[0], dtype=torch.float32) / 255.0        # :31
+    mean = torch.tensor(normalization[0], dtype=batch[0].dtype, device=batch[0].device) / 255.0  # :31
     a, b = batch[0] / 255.0, batch[1] / 255.0                                 # :32-33
     out_hw = a.shape[1:3]
     valid = create_border_mask(a, 0.1)                                         # :38

@@ -124,10 +124,12 @@ def _fp32_frac(f, fl):
     return (f - fl) + (s - (f - fl)).detach()
 
 
-def warp_taps(flow, mode):
+def warp_taps(flow, mode, floor_from=None):
     """Tap pixels and bilinear weights of one gather: mode 0 = BackwardWarp (zero outside), 1 = image_warp
     (clamped taps), 2 = spatial transformer (absolute coordinates, weights from the clamped taps).  Returns
-    [(yy, xx, weight, valid)] for the taps (y0,x0) (y1,x0) (y0,x1) (y1,x1); weights differentiable w.r.t. flow."""
+    [(yy, xx, weight, valid)] for the taps (y0,x0) (y1,x0) (y0,x1) (y1,x1); weights differentiable w.r.t. flow.
+    `floor_from` (mode 1): the flow whose floor() picks the taps, e.g. the fp32 flow a kernel warped with; the
+    weights still come from `flow`, so the float64 derivative is taken on the kernel's side of an integer."""
     B, H, W, _ = flow.shape
     u, v = flow[..., 0], flow[..., 1]
     gx = torch.arange(W, device=flow.device).view(1, 1, W)
@@ -139,7 +141,8 @@ def warp_taps(flow, mode):
         # is discontinuous where the floor changes), with d position / d flow = 1
         x, y = _fp32_sum(gx, u), _fp32_sum(gy, v)
     if mode == 1:
-        fu, fv = torch.floor(u).detach(), torch.floor(v).detach()
+        src = flow if floor_from is None else floor_from.to(flow.dtype)
+        fu, fv = torch.floor(src[..., 0]).detach(), torch.floor(src[..., 1]).detach()
         xw, yw = _fp32_frac(u, fu), _fp32_frac(v, fv)
         x0, y0 = gx + fu.long(), gy + fv.long()
     else:
@@ -162,11 +165,12 @@ def warp_taps(flow, mode):
     return [(cy0, cx0, wl * wt, ones), (cy1, cx0, wl * yb, ones), (cy0, cx1, xr * wt, ones), (cy1, cx1, xr * yb, ones)]
 
 
-def warp(img, flow, mode, skip_tap=None):
+def warp(img, flow, mode, skip_tap=None, floor_from=None):
     """The bilinear gather of unflow_backward_warp_fwd in float64 (differentiable w.r.t. img and flow).
-    `skip_tap`: leave tap t of warp_taps out (a wrong kernel, for the negative control)."""
+    `skip_tap`: leave tap t of warp_taps out (a wrong kernel, for the negative control); `floor_from`: see
+    warp_taps."""
     out = 0
-    for t, (yy, xx, wgt, valid) in enumerate(warp_taps(flow, mode)):
+    for t, (yy, xx, wgt, valid) in enumerate(warp_taps(flow, mode, floor_from)):
         if t != skip_tap:
             out = out + (wgt * valid)[..., None] * _gather(img, yy, xx)
     return out
@@ -511,3 +515,53 @@ def supervised_loss_grads(flow, gt, mask, scale=20.0):
         per_px = m * (1e-5 * c.abs() + dc.abs() * 8 * f32 * (v.abs() + gt.double().abs()))
     budget, = torch.autograd.grad(v, f, grad_outputs=per_px * scale / n)
     return loss.detach(), dflow, budget.abs()
+
+
+# ---- the networks' leaky-ReLU kinks (tests/test_gpu_float64_network.py, tests/test_gpu_float64_objective.py) ----
+def record_kink_sides(monkeypatch):
+    """Record, per layer scope and in call order, which side of the leaky-ReLU kink every element of the product's
+    activations fell on (y > 0).  Returns {scope: [bool masks]}."""
+    from unflow_b200.e2eflow.core import flownet as pfl
+    sides = {}
+    real_conv, real_deconv = pfl._Scope.conv, pfl._Scope.deconv
+
+    def conv(self, x, name, stride=1, act=True, out=None):
+        y = real_conv(self, x, name, stride, act, out)
+        if act:
+            sides.setdefault(self.p + name, []).append(y.detach() > 0)
+        return y
+
+    def deconv(self, x, name, act=True, out=None):
+        y = real_deconv(self, x, name, act, out)
+        if act:
+            sides.setdefault(self.p + name, []).append(y.detach() > 0)
+        return y
+    monkeypatch.setattr(pfl._Scope, "conv", conv)
+    monkeypatch.setattr(pfl._Scope, "deconv", deconv)
+    return sides
+
+
+def follow_kink_sides(monkeypatch, sides):
+    """The oracle's leaky ReLU with the product's side of the kink: where fp32 and float64 disagree on the sign of
+    a pre-activation within rounding of zero, the slope (1 or 0.1) is the one the product took.  Without this a
+    handful of such elements on the 5x18-pixel levels moves a weight gradient by 1e-2.  The product's calls over
+    one 2B batch (both directions, both images) cover the oracle's two calls over B, in the same order."""
+    from oracle import flownet as oflownet
+    cat = {k: torch.cat(v, 0) for k, v in sides.items()}
+    used = dict.fromkeys(cat, 0)
+
+    def act(x, scope):
+        i, n = used[scope], x.shape[0]
+        m = cat[scope][i:i + n]
+        assert m.shape == x.shape, (scope, tuple(m.shape), tuple(x.shape))
+        used[scope] = i + n
+        return torch.where(m, x, 0.1 * x)
+    monkeypatch.setattr(oflownet, "leaky_relu", act)
+    return used, cat
+
+
+def errors(got, ref):
+    """(relative L2 error, max error over max |ref|) of a float32 result against its float64 reference."""
+    d = got.double() - ref
+    return (float(d.norm() / ref.norm().clamp_min(1e-300)),
+            float(d.abs().max() / ref.abs().max().clamp_min(1e-300)))

@@ -22,11 +22,12 @@ Every flow and every variable gradient (weights and biases separately) is scored
 ||got - ref|| / ||ref|| and its max error max|got - ref| / max|ref|; the bound is on the larger of the two.  Variables
 of frozen networks must get no gradient, as in the reference.
 
-The float64 network takes each leaky ReLU's side of the kink from the product's own activations (_follow_kink_sides).
-Where fp32 and float64 disagree on the sign of a pre-activation within rounding of zero, the slopes differ (1 vs
-0.1), and on the coarse levels (5x18 pixels at 320x1152) one such element is a sizeable share of a weight gradient:
-with the float64 network's own signs the gradients differed by up to 2.6e-2 (max) / 3.3e-3 (rel L2), in fp32 mode
-as well (9.6e-3 / 2.2e-3), which would have hidden the reverse-volume control below.
+The float64 network takes each leaky ReLU's side of the kink from the product's own activations
+(float64_refs.follow_kink_sides).  Where fp32 and float64 disagree on the sign of a pre-activation within rounding
+of zero, the slopes differ (1 vs 0.1), and on the coarse levels (5x18 pixels at 320x1152) one such element is a
+sizeable share of a weight gradient: with the float64 network's own signs the gradients differed by up to 2.6e-2
+(max) / 3.3e-3 (rel L2), in fp32 mode as well (9.6e-3 / 2.2e-3), which would have hidden the reverse-volume control
+below.
 
 Measured on an H100 SXM 80 GB (HBM3) at a 700 W power limit (worst rel L2 / max over the tensors):
 
@@ -151,47 +152,6 @@ def _trainable(spec, train_all, names):
     return {n for n in names if n.startswith(root)}
 
 
-def _record_kink_sides(monkeypatch):
-    """Record, per layer scope and in call order, which side of the leaky-ReLU kink every element of the product's
-    activations fell on (y > 0).  Returns {scope: [bool masks]}."""
-    from unflow_b200.e2eflow.core import flownet as pfl
-    sides = {}
-    real_conv, real_deconv = pfl._Scope.conv, pfl._Scope.deconv
-
-    def conv(self, x, name, stride=1, act=True, out=None):
-        y = real_conv(self, x, name, stride, act, out)
-        if act:
-            sides.setdefault(self.p + name, []).append(y.detach() > 0)
-        return y
-
-    def deconv(self, x, name, act=True, out=None):
-        y = real_deconv(self, x, name, act, out)
-        if act:
-            sides.setdefault(self.p + name, []).append(y.detach() > 0)
-        return y
-    monkeypatch.setattr(pfl._Scope, "conv", conv)
-    monkeypatch.setattr(pfl._Scope, "deconv", deconv)
-    return sides
-
-
-def _follow_kink_sides(monkeypatch, sides):
-    """The oracle's leaky ReLU with the product's side of the kink: where fp32 and float64 disagree on the sign of
-    a pre-activation within rounding of zero, the slope (1 or 0.1) is the one the product took.  Without this a
-    handful of such elements on the 5x18-pixel levels moves a weight gradient by 1e-2.  The product's calls over
-    one 2B batch (both directions, both images) cover the oracle's two calls over B, in the same order."""
-    cat = {k: torch.cat(v, 0) for k, v in sides.items()}
-    used = dict.fromkeys(cat, 0)
-
-    def act(x, scope):
-        i, n = used[scope], x.shape[0]
-        m = cat[scope][i:i + n]
-        assert m.shape == x.shape, (scope, tuple(m.shape), tuple(x.shape))
-        used[scope] = i + n
-        return torch.where(m, x, 0.1 * x)
-    monkeypatch.setattr(oflownet, "leaky_relu", act)
-    return used, cat
-
-
 def run_product(case, tfv, inputs, mode="3xtf32"):
     """The product on ``inputs`` (one tuple per pass): (flows of every pass, {name: gradient}, frozen names with
     a gradient).  Gradients are read from the Trainer's flat buffer (plus the L2 term the Adam kernel adds)."""
@@ -271,20 +231,13 @@ def run_oracle(monkeypatch, case, tfv, inputs):
     return all_flows, grads
 
 
-def errors(got, ref):
-    """(relative L2 error, max error over max |ref|)."""
-    d = got.double() - ref
-    return (float(d.norm() / ref.norm().clamp_min(1e-300)),
-            float(d.abs().max() / ref.abs().max().clamp_min(1e-300)))
-
-
 def compare(got_flows, ref_flows, got_grads, ref_grads):
     """{'flow' | 'weights' | 'biases': [(score, rel L2, max, name)]}; a missing gradient scores infinity."""
     rows = {"flow": [], "weights": [], "biases": []}
     for k, (gf, rf) in enumerate(zip(got_flows, ref_flows)):
         assert [n for n, _ in gf] == [n for n, _ in rf]
         for (n, g), (_, r) in zip(gf, rf):
-            l2, mx = errors(g, r)
+            l2, mx = R.errors(g, r)
             rows["flow"].append((max(l2, mx), l2, mx, "pass%d %s" % (k, n)))
     assert set(got_grads) == set(ref_grads), (sorted(set(got_grads) ^ set(ref_grads)))
     for name, r in ref_grads.items():
@@ -293,7 +246,7 @@ def compare(got_flows, ref_flows, got_grads, ref_grads):
         if g is None:
             rows[fam].append((float("inf"), float("inf"), float("inf"), name))
             continue
-        l2, mx = errors(g, r)
+        l2, mx = R.errors(g, r)
         rows[fam].append((max(l2, mx), l2, mx, name))
     return rows
 
@@ -336,10 +289,10 @@ def check_case(monkeypatch, cid, mode="3xtf32"):
     tfv = _variables(case[0], case[2], seed=5)
     inputs = case_inputs(case)
     with monkeypatch.context() as m:
-        sides = _record_kink_sides(m)
+        sides = R.record_kink_sides(m)
         flows, grads, frozen = run_product(case, tfv, inputs, mode=mode)
     with monkeypatch.context() as m:
-        used, cat = _follow_kink_sides(m, sides)
+        used, cat = R.follow_kink_sides(m, sides)
         ref_flows, ref_grads = run_oracle(m, case, tfv, inputs)
     assert all(used[k] == cat[k].shape[0] for k in cat), "activations the oracle did not consume"
     rows = compare(flows, ref_flows, grads, ref_grads)
@@ -394,7 +347,7 @@ def test_evaluation_flows_match_float64(monkeypatch, spec):
                 a, b = im1.double() / 255.0 - mean, im2.double() / 255.0 - mean
                 rfw, rbw = oflownet.flownet(v64, a, b, spec, backward_flow=True)
             for d, got, ref in (("fw", fw, rfw[-1][0]), ("bw", bw, rbw[-1][0])):
-                l2, mx = errors(got, tfc.resize_bilinear_legacy(ref, [H, W]) * (oflownet.FLOW_SCALE * 4))
+                l2, mx = R.errors(got, tfc.resize_bilinear_legacy(ref, [H, W]) * (oflownet.FLOW_SCALE * 4))
                 rows.append((max(l2, mx), l2, mx, "%dx%d %s" % (H, W, d)))
     finally:
         conv_ops.set_mode(prev)
