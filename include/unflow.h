@@ -20,10 +20,9 @@
  *   - re-entrant: safe to call from several host threads on distinct streams.
  *     Process-global state: the atomic launch counter, the thread-local error
  *     string, the once-resolved driver entry point used to encode TMA tensor
- *     maps, and the tuning options set
- *     through unflow_set_int_option() (kernel-variant selectors only -- every
- *     variant computes the same result; set them before launching, not while
- *     other threads launch).
+ *     maps, and the accumulation chunk set through
+ *     unflow_set_int_option() (set it before launching, not while other
+ *     threads launch).
  */
 #ifndef UNFLOW_H_
 #define UNFLOW_H_
@@ -50,12 +49,9 @@ const char *unflow_last_error(void);
  * reset); bench.py reports it as gpu_launches. */
 unsigned long long unflow_launch_count(void);
 void unflow_reset_launch_count(void);
-/* Tuning knobs for tests / benchmarks.  "corr_fwd_variant": 1 (one row pair per thread) or
- * 3 (three row pairs per thread); default 1; results are bit-identical.  "tc_chunk" (1..64): K blocks per
- * tensor-core accumulation of the tc_* kernels, default 8 (the accumulator truncates, so the error grows with
- * the chunk: about 8x at 64); "tc_ksplit" (0 / 1): split the K loop of layers with few
- * tiles; "tc_pair_px" (0 / 1): two output-parity classes per tile in narrow transposed layers;
- * "narrow_fwd_tma" (0 / 1): TMA-staged narrow 3x3 forward. */
+/* Accuracy knob for tests / benchmarks; the only option is "tc_chunk" (1..64): K blocks per tensor-core
+ * accumulation of the tc_* kernels, default 8 (the accumulator truncates, so the error grows with the chunk:
+ * about 8x at 64).  Any other name or value: UNFLOW_EINVAL. */
 int unflow_set_int_option(const char *name, int value);
 
 /* ------------------------------------------------------------------------
@@ -321,11 +317,11 @@ int unflow_conv3x3_narrow_wgrad(const float *x, long long x_pitch, const float *
  * launches add [5]: stages of the ring; tc_wgrad launches add [4]: consumer wait for a free split slot, [5, 6]:
  * raw and split ring slots (csrc/tc_wgrad.cu). */
 int unflow_tc_conv_debug(long long *buf);
-/* unflow_tc_conv_plan (host only, for the CPU tests): the tap / class / tile plan the launcher builds,
- * as integers (layout in csrc/tc_conv.cu); returns the count written, -needed when `cap` is too
- * small, -1 on invalid arguments.  mode | 4: with the two-parity-classes-per-tile rewrite the launcher applies
- * to transposed layers of 33..64 output channels.  The last integer is the number of K slices per tile the
- * launcher uses when the epilogue allows slicing. */
+/* unflow_tc_conv_plan (host only, for the CPU tests): the tap / class / tile plan unflow_tc_conv launches,
+ * as integers (layout in csrc/tc_conv.cu), including the two-parity-classes-per-tile rewrite it applies to
+ * transposed layers of 33..64 output channels; returns the count written, -needed when `cap` is too
+ * small, -1 on invalid arguments.  Only the low two bits of `mode` are read.  The last integer is the
+ * number of K slices per tile the launcher uses when the epilogue allows slicing. */
 int unflow_tc_conv_plan(int N, int Hin, int Win, int Cin, int Hout, int Wout, int Cout, int mode,
                         int stride, int kh, int kw, int pad_t, int pad_l, int *out, int cap);
 int unflow_tc_wsplit(const float *w, float *w_hi, float *w_lo, int taps, int R, int C, long long s_t,

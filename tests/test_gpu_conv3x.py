@@ -221,34 +221,40 @@ def test_narrow_flow_head_and_input_gradient_match_float64(mode3x, N, C, H, W):
 
 
 @pytest.mark.parametrize("N,C,H,W", [(2, 194, 37, 70), (1, 386, 48, 160), (2, 1026, 6, 20), (1, 20, 16, 32)])
-@pytest.mark.parametrize("tma", [1, 0])
-def test_narrow_flow_head_tma_and_cp_async_kernels(mode3x, N, C, H, W, tma):
+@pytest.mark.parametrize("path", ["tma", "cp_async"])
+def test_narrow_flow_head_tma_and_cp_async_kernels(mode3x, N, C, H, W, path):
     """Both implementations of the flow-head kernels (csrc/narrow_conv_tma.cu: TMA-staged NHWC tiles;
-    csrc/narrow_conv.cu: cp.async staging, the fallback for pitches TMA cannot address) on an input that is a
-    channel slice of a pitch-padded NHWC buffer, as the decoder's concat buffers are; against float64."""
-    from unflow_b200 import _native
+    csrc/narrow_conv.cu: cp.async staging, the fallback for pixel pitches TMA cannot address) on an input that is
+    a channel slice of a pitch-padded NHWC buffer, as the decoder's concat buffers are; against float64.  The
+    launcher picks the kernels from the pitch: a multiple of 4 floats takes TMA, any other the cp.async kernels."""
+    from torch.profiler import ProfilerActivity, profile
     from unflow_b200.e2eflow.core import conv_ops
+    tma = path == "tma"
     gen = torch.Generator().manual_seed(C + 7 * H)
-    pitch = (C + 3) // 4 * 4 + 4
+    pitch, c0 = ((C + 3) // 4 * 4 + 4, 4) if tma else ((C if C % 4 == 2 else C + 2), 0)
     buf = torch.randn(N, H, W, pitch, generator=gen)
-    x = buf[..., 4:4 + C].permute(0, 3, 1, 2)
+    x = buf[..., c0:c0 + C].permute(0, 3, 1, 2)
     w = torch.randn(2, C, 3, 3, generator=gen) * 0.1
     b = torch.randn(2, generator=gen)
     g = torch.randn(N, 2, H, W, generator=gen)
     xd, wd, bd = x.double(), w.double().requires_grad_(True), b.double().requires_grad_(True)
     yd = F.conv2d(xd, wd, bd, padding=1)
     yd.backward(g.double())
-    lib = _native.lib()
-    assert lib.unflow_set_int_option(b"narrow_fwd_tma", tma) == 0
-    try:
-        xc = buf.cuda()[..., 4:4 + C].permute(0, 3, 1, 2)
-        wc = w.cuda().contiguous(memory_format=torch.channels_last).requires_grad_(True)
-        bc = b.cuda().requires_grad_(True)
+    xc = buf.cuda()[..., c0:c0 + C].permute(0, 3, 1, 2)
+    wc = w.cuda().contiguous(memory_format=torch.channels_last).requires_grad_(True)
+    bc = b.cuda().requires_grad_(True)
+    gc = g.cuda()
+    torch.cuda.synchronize()
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        torch.ones(4, device="cuda").add_(1)          # a session can miss the activity issued right at its start
         y = conv_ops._NarrowConv3x3.apply(xc, wc, bc)
-        y.backward(g.cuda())
+        y.backward(gc)
         torch.cuda.synchronize()
-    finally:
-        lib.unflow_set_int_option(b"narrow_fwd_tma", 1)
+    names = {e.name for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA}
+    ran = {k: any(k in nm for nm in names) for k in ("narrow_fwd_tma_kernel", "narrow_wgrad_tma_kernel",
+                                                     "narrow_fwd_kernel", "narrow_wgrad_kernel")}
+    assert ran == {"narrow_fwd_tma_kernel": bool(tma), "narrow_wgrad_tma_kernel": bool(tma),
+                   "narrow_fwd_kernel": not tma, "narrow_wgrad_kernel": not tma}, (ran, sorted(names))
     assert rel(y.detach().cpu(), yd.detach()) < 2e-6
     assert rel(wc.grad.cpu(), wd.grad) < 2e-6
     assert rel(bc.grad.cpu(), bd.grad) < 2e-6

@@ -139,21 +139,6 @@ def test_correlation_full_size_properties():
     assert torch.equal(single[0], out[3])
 
 
-def test_correlation_forward_variants_bit_identical():
-    from unflow_b200 import _native
-    lib = _native.lib()
-    a, b = rnd((2, 48, 20, 56), 31).cuda(), rnd((2, 48, 20, 56), 32).cuda()
-    try:
-        assert lib.unflow_set_int_option(b"corr_fwd_variant", 1) == 0
-        o1 = _ops().correlation(a, b)
-        assert lib.unflow_set_int_option(b"corr_fwd_variant", 3) == 0
-        o3 = _ops().correlation(a, b)
-    finally:
-        lib.unflow_set_int_option(b"corr_fwd_variant", 1)     # back to the default variant
-    assert torch.equal(o1, o3)
-    assert lib.unflow_set_int_option(b"corr_fwd_variant", 2) == 1
-
-
 @pytest.mark.parametrize("shape,md", [((2, 48, 20, 56), 20), ((1, 24, 12, 32), 8), ((4, 256, 48, 160), 20)])
 def test_correlation_bidirectional_one_pass(shape, md):
     """Both cost volumes of the bidirectional pass from ONE forward launch (the reverse volume is a

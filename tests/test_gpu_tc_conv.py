@@ -76,14 +76,14 @@ def test_conv_forward(N, Cin, Cout, H, W, k, stride, pads, xp, bias, act, accum)
 
 
 @pytest.mark.parametrize("bias_act,accum,dense", [(True, False, True), (False, True, False), (False, False, False),
-                                                  (True, True, True)])
+                                                  (True, True, True), (True, False, False), (False, False, True),
+                                                  (False, True, True), (True, True, False)])
 def test_conv_k_slices(bias_act, accum, dense):
     """Few tiles, long K loop (the conv6 / conv6_1 shape of the step): the K loop of a tile is cut into slices
     on different CTAs whose partial sums meet in the output through atomics (zeroed first unless accumulating),
     bias + leaky ReLU as a separate pass.  Same result as the float64 convolution; slack channels untouched.
     Accumulating with bias + activation is y += lrelu(conv + b): the separate pass would see y_old + conv, so
-    that combination runs unsliced."""
-    from unflow_b200 import _native
+    that combination runs unsliced, as does bias + activation into a channel slice of a wider output."""
     t = T()
     N, Cin, Cout, H, W, k = 2, 1024, 256, 6, 20, 3
     x, _ = pitched(N, Cin, H, W, Cin, seed=5)
@@ -98,21 +98,11 @@ def test_conv_k_slices(bias_act, accum, dense):
         ref = ref + out.double()
     else:
         out.fill_(float("nan"))
-    planes = t.split_weights(w)
-    res = {}
-    for ks in (1, 0):
-        assert _native.lib().unflow_set_int_option(b"tc_ksplit", ks) == 0
-        o2 = out.clone() if not dense else None
-        dst, dbuf = (out, obuf) if ks == 1 else pitched(N, Cout, H, W, Cout if dense else Cout + 4, seed=1, fill=-3.5)
-        if ks == 0 and not accum:
-            dst.fill_(float("nan"))
-        t.run(x, planes, dst, mode=0, stride=1, kh=k, kw=k, pad_t=1, pad_l=1, bias=b, act=bias_act, accumulate=accum)
-        res[ks] = dst.clone()
-        assert rel(dst, ref) < TOL, ks
-        if not dense:
-            assert bool((dbuf[..., Cout:] == -3.5).all())
-    _native.lib().unflow_set_int_option(b"tc_ksplit", 1)
-    assert rel(res[1], res[0].double()) < 1e-5
+    t.run(x, t.split_weights(w), out, mode=0, stride=1, kh=k, kw=k, pad_t=1, pad_l=1, bias=b, act=bias_act,
+          accumulate=accum)
+    assert rel(out, ref) < TOL
+    if not dense:
+        assert bool((obuf[..., Cout:] == -3.5).all())
 
 
 DECONV = [  # N, Cin, Cout, H, W, k, stride, pad, out_hw, x pitch, bias+act
@@ -297,23 +287,19 @@ def test_launch_from_a_fresh_host_thread():
 
 
 # ---------------------------------------------------------------------------------------------
-# The tuning options of unflow_set_int_option and the launch paths they select.  Every case compares one
-# launch with float64 at TOL; the plan export (unflow_tc_conv_plan) confirms the path the case is meant for.
+# The launch paths unflow_tc_conv picks from a layer's shape, and the accumulation chunk (tc_chunk).  Every case
+# compares one launch with float64 at TOL; the plan export (unflow_tc_conv_plan) confirms the path the case is
+# meant for.
 # ---------------------------------------------------------------------------------------------
-OPTION_DEFAULTS = {"tc_chunk": 8, "tc_pair_px": 1, "tc_ksplit": 1}
-
-
 @contextlib.contextmanager
-def options(**kv):
+def tc_chunk(chunk):
     from unflow_b200 import _native
     lib = _native.lib()
+    assert lib.unflow_set_int_option(b"tc_chunk", chunk) == 0, chunk
     try:
-        for k, v in kv.items():
-            assert lib.unflow_set_int_option(k.encode(), v) == 0, (k, v)
         yield
     finally:
-        for k in kv:
-            lib.unflow_set_int_option(k.encode(), OPTION_DEFAULTS[k])
+        lib.unflow_set_int_option(b"tc_chunk", 8)
 
 
 def real_lib():
@@ -325,10 +311,10 @@ def real_lib():
 
 
 def launch_plan(N, Hin, Win, Cin, Hout, Wout, Cout, mode, stride, kh, kw, pad_t, pad_l):
-    """What unflow_tc_conv does under the current options (the plan with the two-parity-classes rewrite):
-    n_classes, BN, pair_px and the K slices of a launch whose epilogue allows slicing."""
+    """What unflow_tc_conv launches (the plan with the two-parity-classes rewrite): n_classes, BN, pair_px and
+    the K slices of a launch whose epilogue allows slicing."""
     buf = (ctypes.c_int * 1024)()
-    n = real_lib().unflow_tc_conv_plan(N, Hin, Win, Cin, Hout, Wout, Cout, mode | 4, stride, kh, kw, pad_t, pad_l,
+    n = real_lib().unflow_tc_conv_plan(N, Hin, Win, Cin, Hout, Wout, Cout, mode, stride, kh, kw, pad_t, pad_l,
                                        buf, 1024)
     assert n > 0, n
     nt = buf[14]
@@ -339,7 +325,9 @@ def launch_plan(N, Hin, Win, Cin, Hout, Wout, Cout, mode, stride, kh, kw, pad_t,
 def conv_case(mode, N, Cin, Cout, H, W, k, stride, pad, out_hw=None, bias=False, act=False, accum=False, yp=None,
               seed=0):
     """One tc_conv launch against float64.  mode 0: slim.conv2d with pad = (top, bottom, left, right); mode 1: the
-    transposed convolution with padding `pad`, cropped to out_hw.  Returns (max error / max |ref|, launch plan)."""
+    transposed convolution with padding `pad`, cropped to out_hw.  Returns (max error / max |ref|, launch plan);
+    the plan's "launches" counts the kernels the call launched."""
+    from unflow_b200 import _native
     t = T()
     x, _ = pitched(N, Cin, H, W, t.round4(Cin), seed=seed)
     g = torch.Generator().manual_seed(seed + 1)
@@ -370,7 +358,9 @@ def conv_case(mode, N, Cin, Cout, H, W, k, stride, pad, out_hw=None, bias=False,
     else:
         out.fill_(float("nan"))
     p = launch_plan(N, H, W, Cin, Ho, Wo, Cout, mode, stride, k, k, pt, pl)
+    n0 = _native.launch_count()
     t.run(x, planes, out, mode=mode, stride=stride, kh=k, kw=k, pad_t=pt, pad_l=pl, bias=b, act=act, accumulate=accum)
+    p["launches"] = _native.launch_count() - n0
     assert bool((obuf[..., Cout:] == -3.5).all())          # nothing written past C_out
     return rel(out, ref), p
 
@@ -387,7 +377,7 @@ def test_chunk_option_forward(chunk, mode, N, Cin, Cout, H, W, k, stride, pads, 
     """tc_chunk = K blocks per wgmma accumulation: K loops whose length is not a multiple of the chunk end in a
     short chunk; 64 covers a whole slice in one accumulation.  Longer chunks let more truncating accumulator adds
     pile up, so chunks past the default 8 get TOL * chunk / 8 (measured at 64 on an H100: 1.2e-5 and 6.8e-6)."""
-    with options(tc_chunk=chunk):
+    with tc_chunk(chunk):
         err, p = conv_case(mode, N, Cin, Cout, H, W, k, stride, pads, bias=ba, act=ba)
     assert (p["ntaps"] * p["kblocks"]) % 3 and (p["ntaps"] * p["kblocks"]) % 8
     assert err < TOL * max(1, chunk / 8), err
@@ -402,26 +392,30 @@ CHUNK_WGRAD = [  # N, Cin, Cout, H, W, k, stride, pads, x pitch: 10 and 8 K bloc
 @pytest.mark.parametrize("chunk", [1, 3, 8, 64])
 @pytest.mark.parametrize("N,Cin,Cout,H,W,k,stride,pads,xp", CHUNK_WGRAD)
 def test_chunk_option_weight_gradient(chunk, N, Cin, Cout, H, W, k, stride, pads, xp):
-    with options(tc_chunk=chunk):
+    with tc_chunk(chunk):
         test_conv_weight_gradient(N, Cin, Cout, H, W, k, stride, pads, xp)
 
 
-PAIR = [  # mode, N, Cin, Cout, H, W, k, stride, pad, out_hw, bias+act
-    (1, 2, 130, 40, 6, 20, 4, 2, 1, None, True),              # deconvN, 40 channels: masked columns in both halves
-    (1, 2, 64, 64, 8, 12, 4, 2, 1, None, True),
-    (1, 2, 128, 64, 8, 12, 5, 2, 1, (16, 24), False),        # input gradient of 5x5 s2 SAME(1, 2)
-    (1, 2, 128, 40, 8, 12, 5, 2, 1, (16, 24), False),
+PAIR = [  # mode, N, Cin, Cout, H, W, k, stride, pad, out_hw, bias+act, two classes per tile
+    (1, 2, 130, 40, 6, 20, 4, 2, 1, None, True, True),              # deconvN, 40 channels: masked columns in both halves
+    (1, 2, 64, 64, 8, 12, 4, 2, 1, None, True, True),
+    (1, 2, 128, 64, 8, 12, 5, 2, 1, (16, 24), False, True),        # input gradient of 5x5 s2 SAME(1, 2)
+    (1, 2, 128, 40, 8, 12, 5, 2, 1, (16, 24), False, True),
+    # the same layers where each class keeps its own tile: more than 64 or at most 32 channels, or one tile
+    (1, 2, 130, 96, 6, 20, 4, 2, 1, None, True, False),
+    (1, 2, 64, 32, 8, 12, 4, 2, 1, None, True, False),
+    (1, 2, 128, 64, 3, 4, 5, 2, 1, (6, 8), False, False),
+    (1, 2, 128, 40, 2, 6, 4, 2, 1, None, False, False),
 ]
 
 
-@pytest.mark.parametrize("pair", [0, 1])
-@pytest.mark.parametrize("mode,N,Cin,Cout,H,W,k,stride,pad,out_hw,ba", PAIR)
-def test_pair_px_option(pair, mode, N, Cin, Cout, H, W, k, stride, pad, out_hw, ba):
-    """tc_pair_px: narrow (33..64 channel) transposed layers with two or more tiles run two output-parity classes
-    per 128-wide tile (1) or each class on its own 64-wide tile (0)."""
-    with options(tc_pair_px=pair):
-        err, p = conv_case(mode, N, Cin, Cout, H, W, k, stride, pad, out_hw=out_hw, bias=ba, act=ba, yp=Cout + 4)
-    assert p["tiles"] >= 2 and p["pair_px"] == pair and p["n_classes"] == (2 if pair else 4)
+@pytest.mark.parametrize("mode,N,Cin,Cout,H,W,k,stride,pad,out_hw,ba,pair", PAIR)
+def test_pair_px(mode, N, Cin, Cout, H, W, k, stride, pad, out_hw, ba, pair):
+    """Narrow (33..64 channel) stride-2 transposed layers with two or more tiles run two output-parity classes per
+    128-wide tile; other transposed layers run each of the four classes on its own tiles."""
+    err, p = conv_case(mode, N, Cin, Cout, H, W, k, stride, pad, out_hw=out_hw, bias=ba, act=ba, yp=Cout + 4)
+    assert p["pair_px"] == pair and p["n_classes"] == (2 if pair else 4), p
+    assert p["tiles"] >= 2 or not pair
     assert err < TOL, err
 
 
@@ -435,22 +429,28 @@ KSPLIT = {  # mode, N, Cin, Cout, H, W, k, stride, pad, out_hw, bias+act, accumu
     "pair_px": (1, 2, 512, 64, 8, 12, 4, 2, 1, None, True, False, 64),
     # the input gradient added into a channel slice of a wider buffer (a gradient slot)
     "accumulate_pitched": (1, 2, 1024, 256, 6, 20, 3, 1, 1, None, False, True, 260),
+    # the same layers with bias + activation into a channel slice, or added into the output: the separate pass
+    # could not apply them, so each tile runs as one work item
+    "transposed_s1_bias_act_pitched": (1, 2, 1024, 256, 6, 20, 3, 1, 1, None, True, False, 260),
+    "transposed_s2_3x3_bias_act_pitched": (1, 2, 2048, 64, 6, 10, 3, 2, 0, (12, 20), True, False, 68),
+    "pair_px_bias_act_pitched": (1, 2, 512, 64, 8, 12, 4, 2, 1, None, True, False, 68),
+    "accumulate_bias_act": (1, 2, 1024, 256, 6, 20, 3, 1, 1, None, True, True, 256),
 }
 
 
-@pytest.mark.parametrize("ksplit", [0, 1])
 @pytest.mark.parametrize("case", sorted(KSPLIT))
-def test_ksplit_option(ksplit, case):
-    """tc_ksplit: layers with few tiles and long K loops cut each tile's K loop into slices whose partial sums meet
-    in the output through atomics (1), or run one work item per tile (0)."""
+def test_ksplit(case):
+    """Layers with few tiles and long K loops cut each tile's K loop into slices whose partial sums meet in the
+    output through atomics, bias + leaky ReLU following as a second launch; when the epilogue rules that out (bias +
+    activation into a channel slice or added into the output) each tile runs as one work item."""
     mode, N, Cin, Cout, H, W, k, stride, pad, out_hw, ba, accum, yp = KSPLIT[case]
-    with options(tc_ksplit=ksplit):
-        err, p = conv_case(mode, N, Cin, Cout, H, W, k, stride, pad, out_hw=out_hw, bias=ba, act=ba, accum=accum,
-                           yp=yp)
-    assert (p["ksplit"] > 1) == bool(ksplit), p
-    if case == "pair_px":
+    err, p = conv_case(mode, N, Cin, Cout, H, W, k, stride, pad, out_hw=out_hw, bias=ba, act=ba, accum=accum, yp=yp)
+    assert p["ksplit"] > 1, p
+    sliced = not ba or (not accum and yp == Cout)
+    assert p["launches"] == (2 if sliced and ba else 1), p
+    if case.startswith("pair_px"):
         assert p["pair_px"] == 1
-    if case == "transposed_s2_3x3":
+    if case.startswith("transposed_s2_3x3"):
         cs = p["class_start"]
         assert p["n_classes"] == 4 and [cs[i + 1] - cs[i] for i in range(4)] == [4, 2, 2, 1]
     assert err < TOL, err
@@ -497,7 +497,7 @@ def same_sign_error(layer):
 @pytest.mark.parametrize("chunk", [1, 8])
 @pytest.mark.parametrize("layer", ["conv6_1", "conv3_1", "conv3_1_wgrad"])
 def test_same_sign_long_k(layer, chunk):
-    with options(tc_chunk=chunk):
+    with tc_chunk(chunk):
         err = same_sign_error(layer)
     print("same-sign %s tc_chunk=%d: max rel error %.3e" % (layer, chunk, err))
     assert err <= SAME_SIGN_TOL, err

@@ -30,7 +30,7 @@ def lib():
 
 def plan(N, Hin, Win, Cin, Hout, Wout, Cout, mode, stride, k, pad_t, pad_l):
     buf = (ctypes.c_int * 1024)()
-    n = lib().unflow_tc_conv_plan(N, Hin, Win, Cin, Hout, Wout, Cout, mode | 4, stride, k, k, pad_t, pad_l, buf, 1024)
+    n = lib().unflow_tc_conv_plan(N, Hin, Win, Cin, Hout, Wout, Cout, mode, stride, k, k, pad_t, pad_l, buf, 1024)
     assert n > 0, n
     nt = buf[14]
     cs = list(buf[15:15 + buf[0] + 1])

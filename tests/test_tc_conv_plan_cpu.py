@@ -125,33 +125,27 @@ def test_plan_tiles_of_the_flownet_shapes():
         assert util >= want - 1e-9, (H, W, p["TW"], p["TH"], p["TN"], util)
 
 
-def test_k_slices_of_the_flownet_shapes():
+def test_k_slices_at_the_flownet_shapes():
     """The K-slice decision at the FlowNetC geometry (2B = 8 samples): conv6_1 (1024 -> 1024 channels, 3x3 at
     6x20) has 8 tiles x 8 column blocks = 64 work items for 132 SMs and 288 K blocks per tile, so each tile is cut
-    into two slices; conv3 (128 -> 256 channels, 5x5 stride 2 at 48x160) fills the GPU with tiles alone.
-    tc_ksplit = 0 switches slicing off."""
-    lib = _native.lib()
+    into two slices; conv3 (128 -> 256 channels, 5x5 stride 2 at 48x160) fills the GPU with tiles alone."""
     conv6_1 = (8, 6, 20, 1024, 6, 20, 1024, 0, 1, 3, 3, 1, 1)
     conv3 = (8, 96, 320, 128, 48, 160, 256, 0, 2, 5, 5, 1, 1)
     assert plan(*conv6_1)["ksplit"] == 2
     assert plan(*conv3)["ksplit"] == 1
-    try:
-        assert lib.unflow_set_int_option(b"tc_ksplit", 0) == 0
-        assert plan(*conv6_1)["ksplit"] == 1
-    finally:
-        lib.unflow_set_int_option(b"tc_ksplit", 1)
 
 
-def test_tensor_core_options_reject_values_out_of_range():
-    """unflow_set_int_option accepts tc_chunk 1..64 and tc_pair_px / tc_ksplit 0 / 1; anything else is
-    UNFLOW_EINVAL and leaves the setting alone (the plan of conv6_1 keeps its two K slices)."""
+def test_int_option_takes_tc_chunk_only():
+    """unflow_set_int_option accepts tc_chunk 1..64 and no other option (the paired parity classes and the K
+    slices are chosen from the layer's shape); anything else is UNFLOW_EINVAL and leaves the settings alone (the
+    plan of conv6_1 keeps its two K slices)."""
     lib = _native.lib()
-    for name, bad in ((b"tc_chunk", 0), (b"tc_chunk", 65), (b"tc_chunk", -1), (b"tc_pair_px", 2),
-                      (b"tc_pair_px", -1), (b"tc_ksplit", 2), (b"tc_ksplit", -1)):
+    for name, bad in ((b"tc_chunk", 0), (b"tc_chunk", 65), (b"tc_chunk", -1), (b"tc_pair_px", 0),
+                      (b"tc_pair_px", 1), (b"tc_ksplit", 0), (b"tc_ksplit", 1)):
         assert lib.unflow_set_int_option(name, bad) == _native.UNFLOW_EINVAL, (name, bad)
         assert name.decode() in _native.last_error()
     assert plan(8, 6, 20, 1024, 6, 20, 1024, 0, 1, 3, 3, 1, 1)["ksplit"] == 2
-    for name, good, default in ((b"tc_chunk", 1, 8), (b"tc_chunk", 64, 8), (b"tc_pair_px", 0, 1), (b"tc_ksplit", 0, 1)):
+    for name, good, default in ((b"tc_chunk", 1, 8), (b"tc_chunk", 64, 8)):
         assert lib.unflow_set_int_option(name, good) == _native.UNFLOW_OK
         assert lib.unflow_set_int_option(name, default) == _native.UNFLOW_OK
 
@@ -308,13 +302,14 @@ def execute_pair_px(p, x, w_taps, N, Hout, Wout, Cout):
     return out
 
 
-@pytest.mark.parametrize("N,Cin,H,W,Cout,k,pad,out_hw,units", [(2, 5, 9, 12, 40, 4, 1, None, 12), (2, 3, 8, 12, 64, 5, 1, (16, 24), 15),
-                                                              (2, 4, 8, 12, 33, 3, 0, (16, 24), 6)])
+@pytest.mark.parametrize("N,Cin,H,W,Cout,k,pad,out_hw,units", [(2, 5, 9, 12, 40, 4, 1, None, 12), (2, 6, 8, 12, 64, 5, 1, (16, 24), 15),
+                                                              (2, 8, 8, 12, 33, 3, 0, (16, 24), 6), (2, 7, 8, 12, 48, 4, 1, None, 12)])
 def test_two_parity_classes_per_tile_plan(N, Cin, H, W, Cout, k, pad, out_hw, units):
     """Narrow (33..64 channel) transposed layers: the paired plan covers every output exactly once, reproduces
     conv_transpose2d, and needs `units` (input offset, class pair) blocks per channel block where the plain plan has
     k * k (tap, class) blocks: k4 s2 12 instead of 16, 5x5 s2 15 instead of 25, 3x3 s2 6 instead of 9 -- each at
-    N = 128, which costs the tensor core the same as the plain plan's N = 64."""
+    N = 128, which costs the tensor core the same as the plain plan's N = 64.  The plain plan is the one of the
+    same layer over at most 4 input channels, which runs on the FMA pipes (csrc/conv_fma.cu)."""
     g = torch.Generator().manual_seed(k * 5 + Cout)
     x = torch.randn(N, Cin, H, W, generator=g, dtype=torch.float64)
     w = torch.randn(Cin, Cout, k, k, generator=g, dtype=torch.float64)
@@ -324,13 +319,13 @@ def test_two_parity_classes_per_tile_plan(N, Cin, H, W, Cout, k, pad, out_hw, un
         oph, opw = out_hw[0] - Ho, out_hw[1] - Wo
         Ho, Wo = out_hw
     ref = F.conv_transpose2d(x, w, stride=2, padding=pad, output_padding=(max(oph, 0), max(opw, 0)))[:, :, :Ho, :Wo]
-    p = plan(N, H, W, Cin, Ho, Wo, Cout, 1 | 4, 2, k, k, pad, pad)
+    p = plan(N, H, W, Cin, Ho, Wo, Cout, 1, 2, k, k, pad, pad)
     assert p["pair_px"] == 1 and p["ntaps"] == units
-    plain = plan(N, H, W, Cin, Ho, Wo, Cout, 1, 2, k, k, pad, pad)
+    plain = plan(N, H, W, 4, Ho, Wo, Cout, 1, 2, k, k, pad, pad)
     assert plain["pair_px"] == 0 and plain["ntaps"] == k * k and plain["BN"] == 64
     w_taps = w.permute(2, 3, 1, 0).reshape(k * k, Cout, Cin)
     got = execute_pair_px(p, x.permute(0, 2, 3, 1), w_taps, N, Ho, Wo, Cout)
     torch.testing.assert_close(got.permute(0, 3, 1, 2), ref, rtol=1e-12, atol=1e-12)
     # layers it is not meant for keep the plain plan
-    assert plan(N, H, W, Cin, Ho, Wo, 128, 1 | 4, 2, k, k, pad, pad)["pair_px"] == 0
-    assert plan(N, H, W, Cin, Ho, Wo, 16, 1 | 4, 2, k, k, pad, pad)["pair_px"] == 0
+    assert plan(N, H, W, Cin, Ho, Wo, 128, 1, 2, k, k, pad, pad)["pair_px"] == 0
+    assert plan(N, H, W, Cin, Ho, Wo, 16, 1, 2, k, k, pad, pad)["pair_px"] == 0

@@ -113,7 +113,7 @@ def check(run, lengths, grid=GRID, chunk=CHUNK):
 
 def conv_lengths(N, Hin, Win, Cin, Hout, Wout, Cout, mode, stride, k, pt, pl, ksplit=1):
     buf = (ctypes.c_int * 1024)()
-    n = _native.lib().unflow_tc_conv_plan(N, Hin, Win, Cin, Hout, Wout, Cout, mode | 4, stride, k, k, pt, pl, buf, 1024)
+    n = _native.lib().unflow_tc_conv_plan(N, Hin, Win, Cin, Hout, Wout, Cout, mode, stride, k, k, pt, pl, buf, 1024)
     assert n > 0
     ncls, nblk, kblocks = buf[0], buf[11], buf[13]
     cs = list(buf[15:20])

@@ -59,11 +59,8 @@ def main():
     D2 = 441
     nbytes = 4 * B * H * W * (2 * C + D2)
     flops = 2 * B * H * W * C * D2
-    from unflow_b200 import _native
-    for variant in (1, 3):
-        _native.lib().unflow_set_int_option(b"corr_fwd_variant", variant)
-        t = timeit(lambda: ops.correlation(a, b))
-        report("correlation_fwd(v%d) B8 256x48x160 d20" % variant, *t, nbytes, flops)
+    t = timeit(lambda: ops.correlation(a, b))
+    report("correlation_fwd B8 256x48x160 d20", *t, nbytes, flops)
 
     ar, br = a.clone().requires_grad_(True), b.clone().requires_grad_(True)
     out = ops.correlation(ar, br)
@@ -94,8 +91,7 @@ def main():
     report("image_warp bwd (dflow+dimage) B4 384x1280x3", *t, 4 * Bl * h * w * (3 * 3 + 4))
 
     # flow heads at the shapes of the B=4 bidirectional step, input = channel slice of a pitch-padded NHWC buffer
-    # (what the decoder's concat buffers are): TMA-staged kernels (csrc/narrow_conv_tma.cu) and the cp.async ones
-    from unflow_b200 import _native
+    # (what the decoder's concat buffers are): the TMA-staged kernels (csrc/narrow_conv_tma.cu)
     from unflow_b200.e2eflow.core import conv_ops
     for (N, C, hh, ww, tag) in ((8, 194, 96, 320, "flow2"), (8, 386, 48, 160, "flow3")):
         buf = torch.randn(N, hh, ww, (C + 3) // 4 * 4, device="cuda")
@@ -105,20 +101,16 @@ def main():
         g = torch.randn(N, 2, hh, ww, device="cuda").contiguous(memory_format=torch.channels_last)
         nbytes = 4 * N * hh * ww * (C + 2)
         flops = 2 * N * hh * ww * C * 18
-        for tma in (1, 0):
-            assert _native.lib().unflow_set_int_option(b"narrow_fwd_tma", tma) == 0
-            name = "tma" if tma else "cp.async"
-            wr = wgt.clone().requires_grad_(True)
-            with torch.no_grad():
-                t = timeit(lambda: conv_ops._NarrowConv3x3.apply(x, wgt, bias))
-            report("narrow_conv_fwd %s %s" % (tag, name), *t, nbytes, flops)
+        wr = wgt.clone().requires_grad_(True)
+        with torch.no_grad():
+            t = timeit(lambda: conv_ops._NarrowConv3x3.apply(x, wgt, bias))
+        report("narrow_conv_fwd %s" % tag, *t, nbytes, flops)
 
-            def fwd_bwd():
-                y = conv_ops._NarrowConv3x3.apply(x, wr, bias)     # x needs no grad: wgrad + bias grad only
-                y.backward(g)
-            t = timeit(fwd_bwd)
-            report("narrow_conv fwd+wgrad %s %s" % (tag, name), *t, 2 * nbytes, 2 * flops)
-        _native.lib().unflow_set_int_option(b"narrow_fwd_tma", 1)
+        def fwd_bwd():
+            y = conv_ops._NarrowConv3x3.apply(x, wr, bias)     # x needs no grad: wgrad + bias grad only
+            y.backward(g)
+        t = timeit(fwd_bwd)
+        report("narrow_conv fwd+wgrad %s" % tag, *t, 2 * nbytes, 2 * flops)
 
 
 if __name__ == "__main__":

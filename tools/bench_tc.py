@@ -145,8 +145,8 @@ def geometry(lib, name, a):
     if name == "unflow_tc_conv":
         (_, N, Hin, Win, Cin, _, _, _, y, Hout, Wout, Cout, y_pitch, bias, _, act, accumulate, mode, stride, kh, kw,
          pad_t, pad_l, _) = a
-        BN, tiles, ncls, nblk, ks, class_k = conv_plan(lib, (N, Hin, Win, Cin, Hout, Wout, Cout, mode | 4, stride, kh,
-                                                             kw, pad_t, pad_l))
+        BN, tiles, ncls, nblk, ks, class_k = conv_plan(lib, (N, Hin, Win, Cin, Hout, Wout, Cout, mode, stride, kh, kw,
+                                                             pad_t, pad_l))
         # the launcher's rule (csrc/tc_conv.cu, unflow_tc_conv): slice only where the epilogue allows it
         if not ((not bias and not act) or (bias and act and not accumulate and y_pitch == Cout and Cout % 4 == 0)):
             ks = 1

@@ -3,7 +3,6 @@
 #include <cstring>
 
 #include "common.cuh"
-#include "correlation.cuh"
 
 namespace unflow {
 static thread_local char g_err[512] = "";
@@ -16,9 +15,6 @@ void set_error(const char *fmt, ...) {
   va_end(ap);
 }
 int set_tc_chunk(int v);        // tc_conv.cu
-int set_tc_ksplit(int v);       // tc_conv.cu
-int set_tc_pair_px(int v);      // tc_conv.cu
-int set_narrow_fwd_tma(int v);  // narrow_conv.cu
 void count_launch(int n) { g_launches.fetch_add((unsigned long long)n, std::memory_order_relaxed); }
 }  // namespace unflow
 
@@ -28,14 +24,7 @@ const char *unflow_last_error(void) { return unflow::g_err; }
 unsigned long long unflow_launch_count(void) { return unflow::g_launches.load(); }
 void unflow_reset_launch_count(void) { unflow::g_launches.store(0); }
 int unflow_set_int_option(const char *name, int value) {
-  if (name && !strcmp(name, "corr_fwd_variant") && (value == 1 || value == 3)) {
-    unflow::g_corr_fwd_variant = value;
-    return UNFLOW_OK;
-  }
   if (name && !strcmp(name, "tc_chunk") && unflow::set_tc_chunk(value)) return UNFLOW_OK;
-  if (name && !strcmp(name, "tc_ksplit") && unflow::set_tc_ksplit(value)) return UNFLOW_OK;
-  if (name && !strcmp(name, "tc_pair_px") && unflow::set_tc_pair_px(value)) return UNFLOW_OK;
-  if (name && !strcmp(name, "narrow_fwd_tma") && unflow::set_narrow_fwd_tma(value)) return UNFLOW_OK;
   unflow::set_error("unknown option or value: %s=%d", name ? name : "(null)", value);
   return UNFLOW_EINVAL;
 }

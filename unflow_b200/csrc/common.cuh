@@ -33,21 +33,6 @@ inline int check_launch(const char *what) {
 
 constexpr int kNumSMs = 132;  // H100 SXM
 
-// cuTensorMapEncodeTiled is a driver-API call and needs a current context on the calling thread.  A host thread
-// whose first CUDA work is a launcher of this library (autograd's backward worker, for one) has none until a
-// runtime call binds the device's primary context, and the encode then fails with CUDA_ERROR_INVALID_CONTEXT.
-// cudaSetDevice binds it.  Call this before encoding a tensor map.
-inline int bind_primary_context() {
-  int dev = 0;
-  cudaError_t e = cudaGetDevice(&dev);
-  if (e == cudaSuccess) e = cudaSetDevice(dev);
-  if (e != cudaSuccess) {
-    set_error("cannot make the device's primary context current: %s", cudaGetErrorString(e));
-    return UNFLOW_ECUDA;
-  }
-  return UNFLOW_OK;
-}
-
 inline int ceil_div(long long a, long long b) { return (int)((a + b - 1) / b); }
 
 // grid size for a grid-stride pixel-parallel kernel: enough CTAs to fill the

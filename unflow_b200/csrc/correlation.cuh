@@ -19,7 +19,6 @@ int corr_bwd_generic(const float *gout, const float *in0, const float *in1, floa
                      const CorrGeom &g, cudaStream_t s);
 
 // correlation_tiled.cu
-extern int g_corr_fwd_variant;
 bool corr_tiled_supported(const CorrGeom &g);
 int corr_fwd_tiled(const float *in0, const float *in1, float *out, float *out_rev, const CorrGeom &g,
                    cudaStream_t s);

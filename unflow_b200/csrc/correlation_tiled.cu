@@ -28,12 +28,12 @@
 //  * every output element is written exactly once, as float4, by the thread that owns it.
 //
 // Algorithmic bytes: 4*B*H*W*(2C + D^2); FLOPs: 2*B*H*W*C*D^2 (DESIGN.md).
-#include <cuda.h>
-
-#include "common.cuh"
 #include "correlation.cuh"
+#include "tma.cuh"
 
 namespace unflow {
+
+using namespace tc;
 
 namespace ct {
 constexpr int S2 = 2;
@@ -67,54 +67,6 @@ struct Smem {
   short zero_y[MAXPAIRS], zero_p[MAXPAIRS];
 };
 }  // namespace ct
-
-// ------------------------------------------------------------------------------------------
-// PTX helpers (mbarrier + TMA), sm_90a
-// ------------------------------------------------------------------------------------------
-__device__ __forceinline__ unsigned smem_u32(const void *p) {
-  return (unsigned)__cvta_generic_to_shared(p);
-}
-__device__ __forceinline__ void mbar_init(unsigned long long *bar, int count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void mbar_arrive(unsigned long long *bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive_expect_tx(unsigned long long *bar, unsigned bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes)
-               : "memory");
-}
-__device__ __forceinline__ void mbar_wait(unsigned long long *bar, unsigned parity) {
-  const unsigned addr = smem_u32(bar);
-  unsigned done;
-  do {
-    asm volatile(
-        "{\n"
-        " .reg .pred p;\n"
-        " mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n"
-        " selp.u32 %0, 1, 0, p;\n"
-        "}\n"
-        : "=r"(done)
-        : "r"(addr), "r"(parity)
-        : "memory");
-  } while (!done);
-}
-__device__ __forceinline__ void tma_load_4d(void *dst, const CUtensorMap *map, unsigned long long *bar,
-                                            int c0, int c1, int c2, int c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.shared::cluster.global.tile.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4, %5, %6}], [%2];"
-      ::"r"(smem_u32(dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_5d(void *dst, const CUtensorMap *map, unsigned long long *bar,
-                                            int c0, int c1, int c2, int c3, int c4) {
-  asm volatile(
-      "cp.async.bulk.tensor.5d.shared::cluster.global.tile.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4, %5, %6, %7}], [%2];"
-      ::"r"(smem_u32(dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4)
-      : "memory");
-}
 
 // ------------------------------------------------------------------------------------------
 // Forward kernel
@@ -151,7 +103,7 @@ corr_fwd_tiled_kernel(const __grid_constant__ CUtensorMap map0,  // in0 as [B][C
     if (lane == 0) { s_cnt[warp] = __popc(vmask); s_zcnt[warp] = __popc(zmask); }
   }
   if (warp == NCW && lane == 0) {
-    for (int s = 0; s < STAGES; ++s) { mbar_init(&sm.full[s], 1); mbar_init(&sm.empty[s], NCW); }
+    for (int s = 0; s < STAGES; ++s) { mbar_init(s32(&sm.full[s]), 1); mbar_init(s32(&sm.empty[s]), NCW); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
@@ -197,15 +149,15 @@ corr_fwd_tiled_kernel(const __grid_constant__ CUtensorMap map0,  // in0 as [B][C
       for (int it = 0; it < nchunks; ++it) {
         const int s = it % STAGES;
         const unsigned ph = (unsigned)(it / STAGES) & 1u;
-        mbar_wait(&sm.empty[s], ph ^ 1u);
-        mbar_arrive_expect_tx(&sm.full[s], STAGE_BYTES);
+        mbar_wait(s32(&sm.empty[s]), ph ^ 1u);
+        mbar_expect_tx(s32(&sm.full[s]), STAGE_BYTES);
         float *st = sm.stage[s];
         const int c0 = it * CC;
         // in0 parity planes: coords (x, parity, hh, c, b)
-        tma_load_5d(st, &map0, &sm.full[s], x0, 0, ybase >> 1, c0, b);
-        tma_load_5d(st + IN0_PLANE_FLOATS, &map0, &sm.full[s], x0, 1, ybase >> 1, c0, b);
+        tma_5d(s32(st), &map0, s32(&sm.full[s]), x0, 0, ybase >> 1, c0, b);
+        tma_5d(s32(st + IN0_PLANE_FLOATS), &map0, s32(&sm.full[s]), x0, 1, ybase >> 1, c0, b);
         // in1 window: coords (x, y, c, b)
-        tma_load_4d(st + 2 * IN0_PLANE_FLOATS, &map1, &sm.full[s], x0 - S2 * RMAX, Y2, c0, b);
+        tma_4d(s32(st + 2 * IN0_PLANE_FLOATS), &map1, s32(&sm.full[s]), x0 - S2 * RMAX, Y2, c0, b);
       }
     }
     return;
@@ -232,7 +184,7 @@ corr_fwd_tiled_kernel(const __grid_constant__ CUtensorMap map0,  // in0 as [B][C
   for (int it = 0; it < nchunks; ++it) {
     const int s = it % STAGES;
     const unsigned ph = (unsigned)(it / STAGES) & 1u;
-    mbar_wait(&sm.full[s], ph);
+    mbar_wait(s32(&sm.full[s]), ph);
     if (warp_active) {
       const float *p0 = sm.stage[s] + off0;
       const float *p1 = sm.stage[s] + off1;
@@ -267,7 +219,7 @@ corr_fwd_tiled_kernel(const __grid_constant__ CUtensorMap map0,  // in0 as [B][C
       }
     }
     __syncwarp();
-    if (lane == 0) mbar_arrive(&sm.empty[s]);
+    if (lane == 0) mbar_arrive(s32(&sm.empty[s]));
   }
 
   // ---------------- epilogue: each thread stores its 8 x 11 tile ----------------------------
@@ -330,244 +282,14 @@ corr_fold_grad_kernel(const float *__restrict__ g, const float *__restrict__ gre
 }
 
 // ------------------------------------------------------------------------------------------
-// Forward kernel, variant 2: three row pairs per thread.
-//
-// Variant 1 issues 9 LDS.128 per 88 FMAs (9.8 FMA per 128-bit shared load), which makes the shared-memory
-// pipe the limiter rather than the FMA pipe (a 128-bit warp load
-// costs 4 wavefronts even when lanes share addresses, so >= 16 FMA per LDS.128 are needed to be
-// FMA-bound).  Here a thread owns THREE row pairs that share the in1 row (y, y-2, y-4 against the
-// same y2, i.e. p, p+1, p+2), 4 pixels and 11 displacements: the 24-float in1 window is loaded once
-// for 3 x 4 x 11 = 132 FMAs -> 9 LDS.128 per 132 FMAs (14.7).  21 displacement rows = 7 trios per
-// in1 row, 28 trios per work item = 7 consumer warps (lane = trio 0..3, pixel group 0..3,
-// displacement half 0..1).  Same staging, same pipeline, same zero-fill pass as variant 1; every
-// output is still produced by one thread summing channels in ascending order, so v1 and v2 are
-// bit-identical.
-// ------------------------------------------------------------------------------------------
-namespace ct2 {
-using namespace ct;
-constexpr int NTR = 3;                     // row pairs per thread
-constexpr int PX2 = 4;                     // pixels per thread
-constexpr int NCW2 = 7;                    // consumer warps (7*4 = 28 trio slots)
-constexpr int NTHREADS2 = (NCW2 + 1) * 32;
-constexpr int MAXTRIOS = NY2 * ((2 * RMAX + 1 + NTR - 1) / NTR);   // 28
-constexpr int WLEN = PX2 + S2 * (DO - 1);  // 24-float in1 window
-struct Smem2 {
-  float stage[STAGES][STAGE_FLOATS];
-  unsigned long long full[STAGES];
-  unsigned long long empty[STAGES];
-  int ntrios, nzero;
-  short trio_y[MAXTRIOS], trio_y2r[MAXTRIOS], trio_p[MAXTRIOS], trio_n[MAXTRIOS];
-  short zero_y[MAXPAIRS], zero_p[MAXPAIRS];
-};
-}  // namespace ct2
-
-__global__ void __launch_bounds__(ct2::NTHREADS2, 1)
-corr_fwd_tiled3_kernel(const __grid_constant__ CUtensorMap map0, const __grid_constant__ CUtensorMap map1,
-                       float *__restrict__ out, int C, int H, int W, int r, int y2_first) {
-  using namespace ct2;
-  extern __shared__ __align__(1024) unsigned char smem_raw[];
-  Smem2 &sm = *reinterpret_cast<Smem2 *>(smem_raw);
-
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int x0 = blockIdx.x * TX;
-  const int Y2 = y2_first + blockIdx.y * NY2;
-  const int b = blockIdx.z;
-  const int D = 2 * r + 1;
-  const int ybase = Y2 - S2 * RMAX;
-
-  // Work lists, built in parallel: warp y2r scans the 2r+1 displacement rows of in1 row Y2+y2r
-  // (lane <-> p), ballots the valid ones and ranks them; the producer warp meanwhile initialises the
-  // barriers.  (A serial build by one thread cost 4.5 % of the kernel in the first profile.)
-  __shared__ int s_cnt[NY2], s_zcnt[NY2];
-  unsigned vmask = 0, zmask = 0;
-  int my_y = 0;
-  if (warp < NY2) {
-    const int y2 = Y2 + warp;
-    const bool inside = y2 >= 0 && y2 < H;
-    const int p = lane - r;
-    my_y = y2 - S2 * p;
-    const bool ok = lane < D && my_y >= 0 && my_y < H;
-    vmask = __ballot_sync(0xffffffffu, ok && inside);
-    zmask = __ballot_sync(0xffffffffu, ok && !inside);
-    if (lane == 0) { s_cnt[warp] = __popc(vmask); s_zcnt[warp] = __popc(zmask); }
-  }
-  if (warp == NCW2 && lane == 0) {
-    for (int s = 0; s < STAGES; ++s) { mbar_init(&sm.full[s], 1); mbar_init(&sm.empty[s], NCW2); }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  __syncthreads();
-  if (warp < NY2) {
-    int tbase = 0, zbase = 0;
-    for (int k = 0; k < warp; ++k) { tbase += (s_cnt[k] + NTR - 1) / NTR; zbase += s_zcnt[k]; }
-    const unsigned lt = (1u << lane) - 1u;
-    if ((vmask >> lane) & 1u) {
-      const int rank = __popc(vmask & lt), cnt = __popc(vmask);
-      if (rank % NTR == 0) {
-        const int ti = tbase + rank / NTR;
-        sm.trio_y[ti] = (short)my_y; sm.trio_y2r[ti] = (short)warp; sm.trio_p[ti] = (short)lane;
-        sm.trio_n[ti] = (short)min(NTR, cnt - rank);
-      }
-    }
-    if ((zmask >> lane) & 1u) {
-      const int zi = zbase + __popc(zmask & lt);
-      sm.zero_y[zi] = (short)my_y; sm.zero_p[zi] = (short)lane;
-    }
-    if (warp == NY2 - 1 && lane == 0) {
-      sm.ntrios = tbase + (s_cnt[warp] + NTR - 1) / NTR;
-      sm.nzero = zbase + s_zcnt[warp];
-    }
-  }
-  __syncthreads();
-  const int ntrios = sm.ntrios, nzero = sm.nzero;
-  const size_t plane_out = (size_t)H * W;
-  float *outb = out + (size_t)b * D * D * plane_out;
-
-  if (nzero > 0) {
-    const int per_pair = D * (TX / 4);
-    for (int i = tid; i < nzero * per_pair; i += NTHREADS2) {
-      const int zp = i / per_pair, rem = i - zp * per_pair;
-      const int o = rem / (TX / 4), q = rem - o * (TX / 4);
-      const int x = x0 + 4 * q;
-      if (x < W) {
-        float *dst = outb + ((size_t)(sm.zero_p[zp] * D + o)) * plane_out + (size_t)sm.zero_y[zp] * W + x;
-        *reinterpret_cast<float4 *>(dst) = make_float4(0.f, 0.f, 0.f, 0.f);
-      }
-    }
-  }
-  if (ntrios == 0) return;
-
-  const int nchunks = (C + CC - 1) / CC;
-
-  if (warp == NCW2) {
-    if (lane == 0) {
-      for (int it = 0; it < nchunks; ++it) {
-        const int s = it % STAGES;
-        const unsigned ph = (unsigned)(it / STAGES) & 1u;
-        mbar_wait(&sm.empty[s], ph ^ 1u);
-        mbar_arrive_expect_tx(&sm.full[s], STAGE_BYTES);
-        float *st = sm.stage[s];
-        const int c0 = it * CC;
-        tma_load_5d(st, &map0, &sm.full[s], x0, 0, ybase >> 1, c0, b);
-        tma_load_5d(st + IN0_PLANE_FLOATS, &map0, &sm.full[s], x0, 1, ybase >> 1, c0, b);
-        tma_load_4d(st + 2 * IN0_PLANE_FLOATS, &map1, &sm.full[s], x0 - S2 * RMAX, Y2, c0, b);
-      }
-    }
-    return;
-  }
-
-  const int slot = warp * 4 + (lane & 3);
-  const bool active = slot < ntrios;
-  const int ts = active ? slot : 0;
-  const int pxg = (lane >> 2) & 3, og = lane >> 4;
-  const int y = sm.trio_y[ts], y2r = sm.trio_y2r[ts], pidx = sm.trio_p[ts], nrows = active ? sm.trio_n[ts] : 0;
-  const int yrel = y - ybase;
-  // rows of the trio: y, y-2, y-4 -> same parity plane, consecutive (descending) plane rows
-  int off0[NTR];
-#pragma unroll
-  for (int k = 0; k < NTR; ++k) {
-    const int kk = k < nrows ? k : 0;   // unused slots alias row 0 (stay inside the staged tile)
-    off0[k] = (yrel & 1) * IN0_PLANE_FLOATS + ((yrel >> 1) - kk) * P0 + pxg * PX2;
-  }
-  const int off1 = 2 * IN0_PLANE_FLOATS + y2r * WIN + pxg * PX2 + og * (S2 * RMAX);
-
-  float acc[NTR][DO][PX2];
-#pragma unroll
-  for (int k = 0; k < NTR; ++k)
-#pragma unroll
-    for (int t = 0; t < DO; ++t)
-#pragma unroll
-      for (int i = 0; i < PX2; ++i) acc[k][t][i] = 0.0f;
-
-  const bool warp_active = warp * 4 < ntrios;
-  for (int it = 0; it < nchunks; ++it) {
-    const int s = it % STAGES;
-    const unsigned ph = (unsigned)(it / STAGES) & 1u;
-    mbar_wait(&sm.full[s], ph);
-    if (warp_active) {
-      const float *st = sm.stage[s];
-      const float *p1 = st + off1;
-#pragma unroll 2
-      for (int cc = 0; cc < CC; ++cc) {
-        float a[NTR][PX2], w[WLEN];
-#pragma unroll
-        for (int k = 0; k < NTR; ++k) {
-          const float4 v = *reinterpret_cast<const float4 *>(st + off0[k] + cc * (R0H * P0));
-          a[k][0] = v.x; a[k][1] = v.y; a[k][2] = v.z; a[k][3] = v.w;
-        }
-#pragma unroll
-        for (int q = 0; q < WLEN / 4; ++q) {
-          const float4 v = *reinterpret_cast<const float4 *>(p1 + cc * (NY2 * WIN) + 4 * q);
-          w[4 * q] = v.x; w[4 * q + 1] = v.y; w[4 * q + 2] = v.z; w[4 * q + 3] = v.w;
-        }
-#pragma unroll
-        for (int k = 0; k < NTR; ++k)
-#pragma unroll
-          for (int t = 0; t < DO; ++t)
-#pragma unroll
-            for (int i = 0; i < PX2; ++i) acc[k][t][i] = fmaf(a[k][i], w[i + S2 * t], acc[k][t][i]);
-      }
-    }
-    __syncwarp();
-    if (lane == 0) mbar_arrive(&sm.empty[s]);
-  }
-
-  if (active) {
-    const float denom = (float)C;
-    const int x = x0 + pxg * PX2;
-    if (x < W) {
-#pragma unroll
-      for (int k = 0; k < NTR; ++k) {
-        if (k >= nrows) continue;
-        const int yk = y - S2 * k;          // p + k  <->  row y - 2k
-#pragma unroll
-        for (int t = 0; t < DO; ++t) {
-          const int o = og == 0 ? t - RMAX : t;
-          if (o < -r || o > r || (og == 1 && t == 0)) continue;
-          float *dst = outb + ((size_t)((pidx + k) * D + (o + r))) * plane_out + (size_t)yk * W + x;
-          *reinterpret_cast<float4 *>(dst) = make_float4(acc[k][t][0] / denom, acc[k][t][1] / denom,
-                                                         acc[k][t][2] / denom, acc[k][t][3] / denom);
-        }
-      }
-    }
-  }
-}
-
-// ------------------------------------------------------------------------------------------
 // Host side
 // ------------------------------------------------------------------------------------------
-typedef CUresult (*EncodeTiledFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *,
-                                  const cuuint64_t *, const cuuint64_t *, const cuuint32_t *,
-                                  const cuuint32_t *, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-static EncodeTiledFn get_encode_fn() {
-  static EncodeTiledFn fn = nullptr;
-  static bool tried = false;
-  if (!tried) {
-    tried = true;
-    void *p = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess &&
-        q == cudaDriverEntryPointSuccess)
-      fn = (EncodeTiledFn)p;
-  }
-  return fn;
-}
-
 static int encode_map(CUtensorMap *m, const float *base, int rank, const cuuint64_t *dims,
                       const cuuint64_t *strides_bytes, const cuuint32_t *box) {
-  if (bind_primary_context()) return UNFLOW_ECUDA;
-  EncodeTiledFn fn = get_encode_fn();
-  if (!fn) { set_error("cuTensorMapEncodeTiled entry point not available"); return UNFLOW_ECUDA; }
-  cuuint32_t estr[5] = {1, 1, 1, 1, 1};
-  CUresult r = fn(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, (cuuint32_t)rank, (void *)base, dims,
-                  strides_bytes, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE,
-                  CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled failed (%d)", (int)r); return UNFLOW_ECUDA; }
-  return UNFLOW_OK;
+  const cuuint32_t estr[5] = {1, 1, 1, 1, 1};
+  return tc::encode(m, base, rank, dims, strides_bytes, box, estr, CU_TENSOR_MAP_SWIZZLE_NONE,
+                    CU_TENSOR_MAP_L2_PROMOTION_L2_128B);
 }
-
-int g_corr_fwd_variant = 1;   // v3 runs fewer warps, which hide less latency
 
 bool corr_tiled_supported(const CorrGeom &g) {
   return g.ks == 1 && g.s1 == 1 && g.s2 == ct::S2 && g.pad == g.md && g.ngr <= ct::RMAX &&
@@ -613,13 +335,10 @@ int corr_fwd_tiled(const float *in0, const float *in1, float *out, float *out_re
     if (rc) return rc;
   }
   static bool attr_set = false;
-  const int smem_bytes = (int)sizeof(Smem), smem_bytes2 = (int)sizeof(ct2::Smem2);
-  const int variant = out_rev ? 1 : g_corr_fwd_variant;   // 1: pair per thread (default; the bidirectional form), 3: trio per thread
+  const int smem_bytes = (int)sizeof(Smem);
   if (!attr_set) {
     cudaError_t e = cudaFuncSetAttribute(corr_fwd_tiled_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                          smem_bytes);
-    if (e == cudaSuccess)
-      e = cudaFuncSetAttribute(corr_fwd_tiled3_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes2);
     if (e != cudaSuccess) { set_error("correlation smem attribute: %s", cudaGetErrorString(e)); return UNFLOW_ECUDA; }
     attr_set = true;
   }
@@ -627,10 +346,7 @@ int corr_fwd_tiled(const float *in0, const float *in1, float *out, float *out_re
   const int y2_first = -((S2 * r + NY2 - 1) / NY2) * NY2;
   const int y2_end = g.H + S2 * r;  // exclusive
   dim3 grid(ceil_div(g.W, TX), ceil_div(y2_end - y2_first, NY2), g.B);
-  if (variant == 1)
-    corr_fwd_tiled_kernel<<<grid, NTHREADS, smem_bytes, s>>>(map0, map1, out, out_rev, g.C, g.H, g.W, r, y2_first);
-  else
-    corr_fwd_tiled3_kernel<<<grid, ct2::NTHREADS2, smem_bytes2, s>>>(map0, map1, out, g.C, g.H, g.W, r, y2_first);
+  corr_fwd_tiled_kernel<<<grid, NTHREADS, smem_bytes, s>>>(map0, map1, out, out_rev, g.C, g.H, g.W, r, y2_first);
   count_launch();
   return check_launch("correlation_fwd(tiled)");
 }
@@ -702,7 +418,7 @@ corr_bwd_tiled_kernel(const __grid_constant__ CUtensorMap map_src,   // SRC [B][
   const int joff = S2 * (RMAX - r);        // column offset of displacement o=-r inside the staged window
 
   if (tid == 0) {
-    for (int s = 0; s < STAGES; ++s) { mbar_init(&sm.full[s], 1); mbar_init(&sm.empty[s], NPXG); }
+    for (int s = 0; s < STAGES; ++s) { mbar_init(s32(&sm.full[s]), 1); mbar_init(s32(&sm.empty[s]), NPXG); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   for (int i = tid; i < CF::G_FLOATS; i += NTHREADS) sm.zero_tile[i] = 0.0f;
@@ -721,17 +437,17 @@ corr_bwd_tiled_kernel(const __grid_constant__ CUtensorMap map_src,   // SRC [B][
         const bool va = pa <= r && ya < H, vb = pb >= -r && yb < H;
         const int s = it % STAGES;
         const unsigned ph = (unsigned)(it / STAGES) & 1u;
-        mbar_wait(&sm.empty[s], ph ^ 1u);
+        mbar_wait(s32(&sm.empty[s]), ph ^ 1u);
         const unsigned bytes = (unsigned)(S_FLOATS + (va ? D * CF::GW : 0) + (vb ? D * CF::GW : 0)) * 4u;
-        mbar_arrive_expect_tx(&sm.full[s], bytes);
+        mbar_expect_tx(s32(&sm.full[s]), bytes);
         float *st = sm.stage[s];
-        tma_load_4d(st, &map_src, &sm.full[s], x0 - S2 * RMAX, y2, c0, b);
+        tma_4d(s32(st), &map_src, s32(&sm.full[s]), x0 - S2 * RMAX, y2, c0, b);
         if (!G1) {
-          if (va) tma_load_4d(st + S_FLOATS, &map_g, &sm.full[s], x0, ya, (pa + r) * D, b);
-          if (vb) tma_load_4d(st + S_FLOATS + CF::G_FLOATS, &map_g, &sm.full[s], x0, yb, (pb + r) * D, b);
+          if (va) tma_4d(s32(st + S_FLOATS), &map_g, s32(&sm.full[s]), x0, ya, (pa + r) * D, b);
+          if (vb) tma_4d(s32(st + S_FLOATS + CF::G_FLOATS), &map_g, s32(&sm.full[s]), x0, yb, (pb + r) * D, b);
         } else {
-          if (va) tma_load_4d(st + S_FLOATS, &map_g, &sm.full[s], x0 - S2 * RMAX, y2, (r - pa) * D, b);
-          if (vb) tma_load_4d(st + S_FLOATS + CF::G_FLOATS, &map_g, &sm.full[s], x0 - S2 * RMAX, y2, (r - pb) * D, b);
+          if (va) tma_4d(s32(st + S_FLOATS), &map_g, s32(&sm.full[s]), x0 - S2 * RMAX, y2, (r - pa) * D, b);
+          if (vb) tma_4d(s32(st + S_FLOATS + CF::G_FLOATS), &map_g, s32(&sm.full[s]), x0 - S2 * RMAX, y2, (r - pb) * D, b);
         }
         ++it;
       }
@@ -757,7 +473,7 @@ corr_bwd_tiled_kernel(const __grid_constant__ CUtensorMap map_src,   // SRC [B][
     const bool va = pa <= r && ya < H, vb = pb >= -r && yb < H;
     const int s = it % STAGES;
     const unsigned ph = (unsigned)(it / STAGES) & 1u;
-    mbar_wait(&sm.full[s], ph);
+    mbar_wait(s32(&sm.full[s]), ph);
     if (warp_active) {
       const float *S = sm.stage[s] + lane * PITCH + pxg * PXW + joff;
       // a row that does not use this SRC row reads an all-zero tap tile: no branch in the hot loop
@@ -814,7 +530,7 @@ corr_bwd_tiled_kernel(const __grid_constant__ CUtensorMap map_src,   // SRC [B][
       }
     }
     __syncwarp();
-    if (lane == 0) mbar_arrive(&sm.empty[s]);
+    if (lane == 0) mbar_arrive(s32(&sm.empty[s]));
     ++it;
   }
 

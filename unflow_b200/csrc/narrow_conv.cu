@@ -25,8 +25,6 @@
 #include "common.cuh"
 
 namespace unflow {
-int g_narrow_fwd_tma = 1;          // unflow_set_int_option("narrow_fwd_tma"): 1 = TMA-staged forward (default), 0 = cp.async version
-int set_narrow_fwd_tma(int v) { if (v != 0 && v != 1) return 0; g_narrow_fwd_tma = v; return 1; }
 int narrow_fwd_tma(const float *x, long long x_pitch, const float *w, const float *bias, float *y, long long y_pitch,
                    int N, int H, int W, int C, int csplit, cudaStream_t st);     // narrow_conv_tma.cu
 int narrow_wgrad_tma(const float *x, long long x_pitch, const float *g, long long gsN, long long gsC, long long gsH,
@@ -309,10 +307,10 @@ extern "C" int unflow_conv3x3_narrow_fwd(const float *x, long long x_pitch, cons
     cudaError_t e = cudaMemsetAsync(y, 0, sizeof(float) * (size_t)N * H * W * y_pitch, st);
     if (e != cudaSuccess) { set_error("conv3x3_narrow_fwd memset: %s", cudaGetErrorString(e)); return UNFLOW_ECUDA; }
   }
-  if (g_narrow_fwd_tma) {            // TMA-staged version (narrow_conv_tma.cu); -1: arguments it cannot take
-    const int rc = narrow_fwd_tma(x, x_pitch, w, bias, y, y_pitch, N, H, W, C, csplit, st);
-    if (rc >= 0) return rc;
-  }
+  // the TMA-staged version (narrow_conv_tma.cu) takes every call it can; it returns -1 for a base or pixel pitch
+  // that is not 16-byte aligned, weights that do not fit shared memory or a failed encode, and the cp.async
+  // kernel below runs instead
+  if (const int rc = narrow_fwd_tma(x, x_pitch, w, bias, y, y_pitch, N, H, W, C, csplit, st); rc >= 0) return rc;
   const dim3 grid(ceil_div(W, nc::TW), ceil_div(H, nc::TH), N * csplit);
   const size_t smem = (size_t)(nc::KC * nc::FWD_CHS + nc::KC * 24) * sizeof(float);
   nc::narrow_fwd_kernel<<<grid, nc::THREADS, smem, st>>>(x, w, bias, y, H, W, C, x_pitch, y_pitch, csplit);
@@ -345,8 +343,7 @@ extern "C" int unflow_conv3x3_narrow_wgrad(const float *x, long long x_pitch, co
   const dim3 grid(ceil_div(W, nc::TW), ceil_div(H, nc::TH), N * csplit);
   const size_t smem = (size_t)(nc::KC * (nc::SR * nc::PITCH + 1) + nc::TH * nc::GPITCH) * sizeof(float);
   float *part = (float *)workspace;
-  int rc_tma = -1;
-  if (g_narrow_fwd_tma) rc_tma = narrow_wgrad_tma(x, x_pitch, g, gsN, gsC, gsH, gsW, part, N, H, W, C, csplit, s);
+  const int rc_tma = narrow_wgrad_tma(x, x_pitch, g, gsN, gsC, gsH, gsW, part, N, H, W, C, csplit, s);
   if (rc_tma > 0) return rc_tma;
   if (rc_tma < 0) {
     nc::narrow_wgrad_kernel<<<grid, nc::THREADS, smem, s>>>(x, g, gsN, gsC, gsH, gsW, part, H, W, C, x_pitch, csplit);

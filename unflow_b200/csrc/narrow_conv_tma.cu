@@ -13,7 +13,7 @@
 // The layer's weights are staged once per CTA as [chunk][output][tap][16].
 // Small images (flow4..flow6: 8..48 tiles on 132 SMs) split the channel chunks over several CTAs per tile that
 // add their parts with atomics into a zeroed output, as narrow_fwd_kernel does.
-#include "tc_common.cuh"
+#include "tma.cuh"
 
 namespace unflow {
 namespace nct {

@@ -1,9 +1,7 @@
-// tc_common.cuh -- PTX wrappers (mbarrier, TMA, wgmma) and the tensor-map encoder shared by the tensor-core
-// kernels (tc_conv.cu: forward / input gradient, tc_wgrad.cu: weight gradient).
+// tc_common.cuh -- PTX wrappers (wgmma, register budgets, barriers) and the stream-K segment walk shared by the
+// tensor-core kernels (tc_conv.cu: forward / input gradient, tc_wgrad.cu: weight gradient).
 #pragma once
-#include <cuda.h>
-
-#include "common.cuh"
+#include "tma.cuh"
 #include "tc_schedule.h"
 
 namespace unflow {
@@ -23,52 +21,8 @@ extern long long *g_dbg;               // tc_conv.cu: role-timer buffer (unflow_
 extern int g_chunk;                    // tc_conv.cu: K blocks per wgmma accumulation between register adds (default CHUNK)
 
 // ------------------------------------------------------------------------------------------
-// PTX helpers
+// PTX helpers (the mbarrier and TMA ones are in tma.cuh)
 // ------------------------------------------------------------------------------------------
-__device__ __forceinline__ unsigned s32(const void *p) { return (unsigned)__cvta_generic_to_shared(p); }
-
-__device__ __forceinline__ void mbar_init(unsigned bar, int count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count));
-}
-__device__ __forceinline__ void mbar_arrive(unsigned bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void mbar_expect_tx(unsigned bar, unsigned bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(unsigned bar, unsigned parity) {
-  unsigned done;
-  do {
-    asm volatile(
-        "{\n .reg .pred p;\n mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n"
-        " selp.u32 %0, 1, 0, p;\n}\n"
-        : "=r"(done) : "r"(bar), "r"(parity) : "memory");
-  } while (!done);
-}
-// One lane of a fully converged warp (elect.sync): the TMA producer runs its loop with all lanes converged and
-// issues under this predicate.
-__device__ __forceinline__ bool elect_one() {
-  unsigned pred = 0;
-  asm volatile("{\n .reg .pred p;\n elect.sync _|p, 0xFFFFFFFF;\n selp.u32 %0, 1, 0, p;\n}\n" : "=r"(pred));
-  return pred != 0;
-}
-__device__ __forceinline__ void tma_4d(unsigned dst, const CUtensorMap *map, unsigned bar, int c0, int c1,
-                                       int c2, int c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.shared::cluster.global.tile.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4, %5, %6}], [%2];"
-      ::"r"(dst), "l"(map), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
-}
-__device__ __forceinline__ void tma_3d(unsigned dst, const CUtensorMap *map, unsigned bar, int c0, int c1,
-                                       int c2) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.shared::cluster.global.tile.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4, %5}], [%2];"
-      ::"r"(dst), "l"(map), "r"(bar), "r"(c0), "r"(c1), "r"(c2) : "memory");
-}
-__device__ __forceinline__ void fence_proxy_async() {
-  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-}
 // register budget of the calling warp; every warp of a warpgroup must run the same one
 template <int N>
 __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
@@ -206,37 +160,6 @@ __device__ __forceinline__ Segment segment_at(const SkSchedule &s, const Segment
   sg.k0 = q == w.n_dp ? s.sk_k[g] : 0;
   sg.k1 = j == s.sk_item[g + 1] ? s.sk_k[g + 1] : -1;
   return sg;
-}
-
-// ---- host: tensor maps --------------------------------------------------------------------------
-typedef CUresult (*EncodeTiledFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *,
-                                  const cuuint64_t *, const cuuint32_t *, const cuuint32_t *,
-                                  CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion,
-                                  CUtensorMapFloatOOBfill);
-inline EncodeTiledFn encode_fn() {
-  static EncodeTiledFn fn = nullptr;
-  static bool tried = false;
-  if (!tried) {
-    tried = true;
-    void *ptr = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &ptr, cudaEnableDefault, &q) == cudaSuccess &&
-        q == cudaDriverEntryPointSuccess)
-      fn = (EncodeTiledFn)ptr;
-  }
-  return fn;
-}
-inline int encode(CUtensorMap *m, const float *basep, int rank, const cuuint64_t *dims,
-                  const cuuint64_t *strides_bytes, const cuuint32_t *box, const cuuint32_t *estr,
-                  CUtensorMapSwizzle swizzle = CU_TENSOR_MAP_SWIZZLE_128B) {
-  if (bind_primary_context()) return UNFLOW_ECUDA;
-  EncodeTiledFn fn = encode_fn();
-  if (!fn) { set_error("cuTensorMapEncodeTiled entry point not available"); return UNFLOW_ECUDA; }
-  CUresult r = fn(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, (cuuint32_t)rank, (void *)basep, dims, strides_bytes, box,
-                  estr, CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle,
-                  CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled failed (%d)", (int)r); return UNFLOW_ECUDA; }
-  return UNFLOW_OK;
 }
 
 }  // namespace tc

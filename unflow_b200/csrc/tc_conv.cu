@@ -417,8 +417,6 @@ wsplit_kernel(const float *__restrict__ w, float *__restrict__ hi, float *__rest
 static int floordiv(int a, int b) { return (a >= 0) ? a / b : -((-a + b - 1) / b); }
 
 int g_chunk = CHUNK;     // unflow_set_int_option("tc_chunk"): K blocks per wgmma accumulation
-int g_pair_px = 1;       // unflow_set_int_option("tc_pair_px"): 1 = narrow transposed layers compute two parity classes per tile
-int g_ksplit = 1;        // unflow_set_int_option("tc_ksplit"): 1 = layers with few tiles cut their K loops into slices, 0 = never
 long long *g_dbg = nullptr;   // unflow_tc_conv_debug: device buffer of 16 long longs for the role timers of CTA 0
 
 // Stream-K fixup storage, per device, allocated on first use and kept: 2 partial-sum slots per CTA (its first and
@@ -477,7 +475,6 @@ static int launch(const CUtensorMap &mA, const CUtensorMap &mBh, const CUtensorM
 
 // K slices for a layer with few tiles and long K loops (work items <= half of the SMs): how many
 inline int choose_ksplit(const ConvParams &p) {
-  if (!g_ksplit) return 1;
   const long long items = (long long)p.n_classes * p.tiles_n * p.tiles_y * p.tiles_x * p.n_blocks;
   if (2 * items > kNumSMs) return 1;
   int min_iters = 1 << 30;
@@ -503,8 +500,6 @@ static int launch_bn(int BN, const CUtensorMap &mA, const float *w_hi, const flo
 
 }  // namespace tc
 int set_tc_chunk(int v) { if (v < 1 || v > 64) return 0; tc::g_chunk = v; return 1; }
-int set_tc_ksplit(int v) { if (v != 0 && v != 1) return 0; tc::g_ksplit = v; return 1; }
-int set_tc_pair_px(int v) { if (v != 0 && v != 1) return 0; tc::g_pair_px = v; return 1; }
 }  // namespace unflow
 
 using namespace unflow;
@@ -589,7 +584,7 @@ static int make_plan(tc::ConvParams &p, int &BN, int N, int Hin, int Win, int Ci
 // tile is TMA zero fill.  Each activation box is loaded and split once for both classes, and a channel block
 // walks fewer K blocks over all classes: k4 s2 12 instead of 16, 5x5 s2 15 instead of 25.
 static bool pair_px_plan(tc::ConvParams &p, int &BN, int mode, int stride, int Cout) {
-  if (!tc::g_pair_px || mode != 1 || stride != 2 || p.n_classes != 4) return false;
+  if (mode != 1 || stride != 2 || p.n_classes != 4) return false;
   if (Cout <= 32 || Cout > 64 || (long long)p.tiles_n * p.tiles_y * p.tiles_x < 2) return false;
   tc::Tap taps[tc::MAX_TAPS];
   int start[3], nt = 0;
@@ -627,21 +622,21 @@ static bool pair_px_plan(tc::ConvParams &p, int &BN, int mode, int stride, int C
 // first consumer thread blocked on the TMA data, [3] its total, [5] the stages of the ring.
 extern "C" int unflow_tc_conv_debug(long long *buf) { tc::g_dbg = buf; return UNFLOW_OK; }
 
-// Debug / test hook: the plan as integers --
+// Debug / test hook: the plan unflow_tc_conv launches, as integers --
 // [n_classes, s_in, s_out, Hit, Wit, TW, TH, TN, tiles_x, tiles_y, tiles_n, n_blocks, BN, kblocks, ntaps,
 //  class_start[5], (class_px, class_py)[4], (dx, dy, widx)[ntaps], pair_px, widx2[ntaps], ksplit]; returns the
-// count written.  ksplit: the K slices the launcher cuts each tile into when the epilogue allows slicing (no bias
-// and no activation, or both on a dense output that is not accumulated into), under the current tc_* options.
+// count written.  pair_px = 1: a narrow transposed layer computes two parity classes per tile (pair_px_plan), and
+// widx2 holds the px = 1 class's tap per input offset.  ksplit: the K slices the launcher cuts each tile into when
+// the epilogue allows slicing (no bias and no activation, or both on a dense output that is not accumulated into).
 extern "C" int unflow_tc_conv_plan(int N, int Hin, int Win, int Cin, int Hout, int Wout, int Cout, int mode,
                                    int stride, int kh, int kw, int pad_t, int pad_l, int *out, int cap) {
-  // mode | 4: also apply the two-parity-classes-per-tile rewrite the launcher uses for narrow transposed layers
-  // (pair_px_plan); pair_px = 1 then, and widx2 holds the px = 1 class's tap per input offset
-  const int want_pair = (mode >> 2) & 1;
+  // bits above the first two are ignored, as they always were: callers written when bit 2 asked for the
+  // two-parity-classes rewrite get the plan they asked for, which is now the only one
   mode &= 3;
   tc::ConvParams p{};
   int BN = 0;
   if (make_plan(p, BN, N, Hin, Win, Cin, Hout, Wout, Cout, mode, stride, kh, kw, pad_t, pad_l)) return -1;
-  if (want_pair) pair_px_plan(p, BN, mode, stride, Cout);
+  if (Cin > 4) pair_px_plan(p, BN, mode, stride, Cout);   // unflow_tc_conv hands Cin <= 4 to conv_fma first
   const int nt = p.class_start[p.n_classes];
   const int need = 15 + 5 + 8 + 3 * nt + 1 + nt + 1;
   if (!out || cap < need) return -need;

@@ -44,14 +44,6 @@ LRELU_SLOPE = 0.1   # _leaky_relu: tf.maximum(0.1 * x, x)  (reference flownet.py
 
 
 # ---------------------------------------------------------------------------------------------
-# Backward checkpoints: the network marks a few activations ("everything created after this point
-# has finished its backward pass once the gradient arrives here"); the data-parallel trainer hangs
-# the all-reduce of the corresponding slice of the flat gradient buffer on them, so the reduction
-# of the decoder / encoder gradients overlaps the rest of the backward pass (core/train.py).
-# ---------------------------------------------------------------------------------------------
-_backward_point_cb = None
-
-# ---------------------------------------------------------------------------------------------
 # Gradient slots: an activation with several consumers (conv5_1 feeds conv6 AND concat5; a concat buffer
 # feeds the next deconv AND a flow head) receives one gradient per consumer, and autograd adds them with a
 # generic strided elementwise kernel (0.5 ms per step in the CUPTI table).  The tensor-core input-gradient
@@ -84,33 +76,6 @@ def grad_slot_get(gen, x, key=None):
 def grad_slot_put(gen, key_or_tensor, g):
     key = key_or_tensor if isinstance(key_or_tensor, tuple) else _slot_key(key_or_tensor)
     _grad_slots.setdefault(gen, {})[key] = g
-
-
-def set_backward_point_callback(fn):
-    """fn(name) is called from inside the backward pass; None removes it."""
-    global _backward_point_cb
-    _backward_point_cb = fn
-
-
-class _BackwardPoint(torch.autograd.Function):
-    @staticmethod
-    def forward(ctx, x, name):
-        ctx.name = name
-        return x.view_as(x)
-
-    @staticmethod
-    def backward(ctx, g):
-        if _backward_point_cb is not None:
-            _backward_point_cb(ctx.name)
-        return g, None
-
-
-def backward_point(x, name):
-    """Identity; with a callback installed and a differentiable ``x`` it reports when the backward pass
-    comes back through this activation."""
-    if _backward_point_cb is None or not x.requires_grad:
-        return x
-    return _BackwardPoint.apply(x, name)
 
 
 def _bias_grad(g, act):

@@ -311,7 +311,6 @@ def _flownet_upconv(s, conv6_1, conv5_1, conv4_1, conv3_1, conv2, conv1=None, in
                     channel_mult=1, full_res=False, channels=2, cats=None):
     slot = (lambda lvl: cats[lvl].slots[1]) if cats else (lambda lvl: None)
     buf = (lambda lvl: cats[lvl].buf) if cats else (lambda lvl: None)
-    conv6_1 = conv_ops.backward_point(conv6_1, s.p + 'decoder')     # decoder gradients complete behind this point
     flow6 = s.conv(conv6_1, 'flow6', act=False)
     deconv5 = s.deconv(conv6_1, 'deconv5', out=slot(5))
     flow6_up5 = s.deconv(flow6, 'flow6_up5', act=False)
@@ -369,7 +368,6 @@ def flownet_s(inputs, channel_mult=1, full_res=False, _scope=None):
     first = (lambda lvl: cats[lvl].slots[0]) if cats else (lambda lvl: None)
     conv2 = s.conv(conv1, 'conv2', 2, out=first(2))
     conv3 = s.conv(conv2, 'conv3', 2)
-    conv3 = conv_ops.backward_point(conv3, s.p + 'trunk')
     conv3_1 = s.conv(conv3, 'conv3_1', out=first(3))
     conv4 = s.conv(conv3_1, 'conv4', 2)
     conv4_1 = s.conv(conv4, 'conv4_1', out=first(4))
@@ -392,7 +390,7 @@ def flownet_c_features(im, channel_mult=1, reuse=None, _scope=None, _conv2_out=N
 
 
 def _flownet_c_trunk(s, conv_redir_and_corr, conv2_a, channel_mult, full_res, cats=None):
-    x = conv_ops.backward_point(conv_redir_and_corr, s.p + 'trunk')   # conv3_1 .. conv6_1 complete behind this point
+    x = conv_redir_and_corr
     if cats is None:
         cats = _decoder_cats(s, x, x.shape[0], (x.shape[2], x.shape[3]), (conv2_a.shape[2], conv2_a.shape[3]),
                              conv2_a.shape[1])

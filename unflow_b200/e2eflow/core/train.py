@@ -87,9 +87,6 @@ class Trainer:
         train.py:160,169).  run.py trains with it on; bench.py and the parity tests keep it off
         (random draws cannot be parity-pinned).  The draws come from the device generator so the
         step stays capturable in a CUDA graph."""
-        # bucketed all-reduce on a side stream behind the backward checkpoints: OFF by default -- the persistent
-        # conv kernels hold every SM, so NCCL's kernels wait for them either way
-        self.overlap_allreduce = __import__('os').environ.get('UNFLOW_OVERLAP_ALLREDUCE', '0') != '0'
         self.augment = bool(augment)
         if self.augment:
             from . import augment as _aug
@@ -126,11 +123,11 @@ class Trainer:
         self._graph = None
         # keep the tracked images of every step for image summaries (unsupervised.tracked_images)
         self.track_images = False
-        # L2 regularisation gradient inside the Adam kernel (CUDA only; UNFLOW_L2_IN_ADAM=0: autograd forms it).
+        # L2 regularisation gradient inside the Adam kernel (CUDA only; on the CPU autograd forms it).
         # flat_grad then holds the gradient of the data terms only -- l2_gradient() is the missing part.
         self.l2_mask = None
         self.l2_scale = float(self.variables.L2_SCALE)
-        if self.device.type == 'cuda' and __import__('os').environ.get('UNFLOW_L2_IN_ADAM', '1') != '0':
+        if self.device.type == 'cuda':
             isw, packed = l2_mask_bytes(self.flat_param.numel(), self._offsets, [p.numel() for p in self.trainable],
                                         [name.endswith('/weights') for name in self.trainable_names])
             self.l2_mask = packed.to(self.device)
@@ -210,62 +207,6 @@ class Trainer:
             return 1.0 / self.world_size
         return 1.0
 
-    # -- gradient all-reduce overlapped with the backward pass ---------------------------------------
-    def _bucket_plan(self):
-        """Cut the flat gradient buffer where the network's backward checkpoints (conv_ops.backward_point)
-        say a suffix of it is final: the variables are laid out in forward order, the backward pass
-        finishes them from the back -- first the decoder (flow6 .. flow2, deconv5 .. deconv2), then
-        conv3_1 .. conv6_1, last the feature layers.  {checkpoint name: (start, end)} in floats; the
-        head of the buffer [0, first start) is reduced after the backward pass."""
-        n_nets = len(self.params.get('flownet', 'S'))
-        if not (n_nets == 1 or not self.params.get('train_all')):
-            return None                                   # several trained networks: keep the single all-reduce
-        names, offs = self.trainable_names, self._offsets
-        scope = names[0].rsplit('/', 2)[0] + '/' if names else ''
-
-        def first(pred):
-            for nm, off in zip(names, offs):
-                if pred(nm):
-                    return off
-            return None
-        dec = first(lambda nm: '/flow6/' in nm)
-        trunk = first(lambda nm: '/conv3_1/' in nm)
-        if dec is None or trunk is None or not trunk < dec:
-            return None
-        net = [nm for nm in names if '/conv3_1/' in nm][0].split('conv3_1/')[0]      # e.g. 'flownet_c/'
-        end = self.flat_grad.numel()
-        return {net + 'decoder': (dec, end), net + 'trunk': (trunk, dec)}, trunk
-
-    def _backward_overlapped(self, loss):
-        """loss.backward() with the all-reduce of each finished slice of the flat gradient buffer launched
-        from the backward checkpoints (NCCL runs on its own stream; the compute stream only waits for the
-        handles before Adam)."""
-        from . import conv_ops
-        plan = self._bucket_plan()
-        if plan is None:
-            loss.backward()
-            self.reduce_gradients()
-            return
-        buckets, head_end = plan
-        works, done = [], set()
-
-        def on_point(name):
-            if name in buckets and name not in done:
-                done.add(name)
-                a, b = buckets[name]
-                works.append(dist.all_reduce(self.flat_grad[a:b], op=dist.ReduceOp.SUM, group=self.pg, async_op=True))
-        conv_ops.set_backward_point_callback(on_point)
-        try:
-            loss.backward()
-        finally:
-            conv_ops.set_backward_point_callback(None)
-        for name, (a, b) in buckets.items():               # a checkpoint that never fired: reduce its slice now
-            if name not in done:
-                works.append(dist.all_reduce(self.flat_grad[a:b], op=dist.ReduceOp.SUM, group=self.pg, async_op=True))
-        works.append(dist.all_reduce(self.flat_grad[:head_end], op=dist.ReduceOp.SUM, group=self.pg, async_op=True))
-        for w in works:
-            w.wait()
-
     def l2_gradient(self):
         """The regularisation gradient the Adam kernel adds (zeros when autograd forms it instead)."""
         if self.l2_mask is None:
@@ -294,11 +235,8 @@ class Trainer:
     def _step_impl(self, *batch):
         """forward + loss + backward + gradient mean + Adam, hyper-parameters from device memory."""
         loss = self.loss(*batch)
-        if self.world_size > 1 and self.overlap_allreduce:
-            self._backward_overlapped(loss)
-        else:
-            loss.backward()
-            self.reduce_gradients()
+        loss.backward()
+        self.reduce_gradients()
         from ..ops import kernel_timer
         with torch.cuda.device(self.device), kernel_timer.span("adam", 32 * self.flat_param.numel()):
             check(_native.lib().unflow_adam_step_dev_l2(
@@ -403,12 +341,8 @@ class Trainer:
             self.graph_replays += 1
             return self._static_loss
         loss = self.loss(*batch)
-        if self.world_size > 1 and self.overlap_allreduce:
-            self._backward_overlapped(loss)
-            scale = 1.0 / self.world_size
-        else:
-            loss.backward()   # accumulates into the flat gradient views
-            scale = self.reduce_gradients()
+        loss.backward()   # accumulates into the flat gradient views
+        scale = self.reduce_gradients()
         self.apply_update(lr, scale)
         return loss.detach()
 
