@@ -371,7 +371,7 @@ def read_scalars(values):
     return {k: out[k] for k in values}
 
 
-def evaluate(variables, params, normalization, examples, eval_size=(384, 1280), loss_averages=None):
+def evaluate(variables, params, normalization, examples, eval_size=(384, 1280), loss_averages=None, pages=None):
     """The checkpoint-evaluation loop of the reference Trainer (train.py:265-385) without the TF
     session / summary scaffolding.
 
@@ -383,7 +383,8 @@ def evaluate(variables, params, normalization, examples, eval_size=(384, 1280), 
     'occluded' (all valid) and 'non-occluded' masks (train.py:314-321).  Returns the dict of
     averages plus the last example's visualisation tensors (train.py:290-293).  ``loss_averages``: a
     dict that receives every tracked loss of ``unsupervised_loss`` averaged over the examples
-    (train.py:323-328), {op name: float}."""
+    (train.py:323-328), {op name: float}.  ``pages``: a ``pages.Tiles`` that receives every example's
+    visualisation tensors as uint8 (the reference's interactive plot, train.py:378-384)."""
     from . import flow_util, tf_image
     from .flow_io import resize_output_flow
     from .image_warp import image_warp
@@ -414,6 +415,9 @@ def evaluate(variables, params, normalization, examples, eval_size=(384, 1280), 
                       'occ': 1 - (1 - occlusion(flow, flow_bw)[0]) * create_outgoing_mask(flow),
                       'reverse disocc': forward_warp(flow_bw) < DISOCC_THRESH,
                       'flow error': flow_util.flow_error_image(flow, flow_occ, mask_occ, mask_noc)}
+            if pages is not None and pages.wants_more():
+                from .pages import to_uint8
+                pages.add(list(images), [to_uint8(v * 255) for v in images.values()])
     out = {k: v / max(n, 1) for k, v in sums.items()}
     out['num_examples'] = n
     if loss_averages is not None:

@@ -22,7 +22,10 @@ nothing for variants with other / no ground truth.  ``--output_benchmark`` write
 ``<out>/<ex>/%06d_10.png`` 16-bit KITTI flow files (``flow_to_int16``: u*64+2^15 clamped and
 truncated, validity 1 -- eval_gui.py:67-73) or ``.flo`` with ``--no-output_png``;
 ``--output_backward`` adds ``_01`` files; ``--output_visual`` writes overlay / flow-colour / error
-images.  The GUI pages (``e2eflow.gui.display``) are out of scope.
+images.  ``--output_pages`` writes the pages the reference's viewer (``e2eflow.gui.display``) shows, for
+the first ``--num_vis`` examples, as ``<out>/pages/%06d.png`` (``core/pages.py``): a row per image slot,
+a column per experiment; its tiles equal the ``--output_visual`` files of the same slots.  The
+interactive Tk window itself is out of scope.
 """
 import argparse
 import os
@@ -116,12 +119,18 @@ def network_flow_fn(params, normalization, variables):
 
 
 def evaluate_examples(name, items, dims, flow_fn, device, num=10, out_dir=None, output_benchmark=False,
-                      output_visual=False, output_backward=False, output_png=True, log=sys.stdout):
+                      output_visual=False, output_backward=False, output_png=True, log=sys.stdout, pages=None):
     """The per-example loop of ``_evaluate_experiment`` (eval_gui.py:110-310).  ``items`` yields what
     the input classes deliver: ``(im1, im2, input_shape[, flow_occ, mask_occ, flow_noc, mask_noc |
-    flow_gt, mask])`` padded / cropped to ``dims``.  Returns ``{scalar name: average}``."""
+    flow_gt, mask])`` padded / cropped to ``dims``.  Returns ``{scalar name: average}``.  ``pages``: a
+    ``core.pages.Tiles`` that receives the uint8 image slots of the examples it still wants, at file size:
+    overlay, brightness error (``|im1 - image_warp(im2, flow)|``), flow and flow error with KITTI / Sintel
+    ground truth; overlay, brightness error, flow and gt with FlyingChairs / Middlebury ground truth;
+    first image, warp error and flow prediction without."""
     from .e2eflow.core import flow_util
     from .e2eflow.core.flow_io import resize_output_flow, write_flo
+    from .e2eflow.core.image_warp import image_warp
+    from .e2eflow.core.pages import to_uint8
     from .e2eflow.core.input import resize_image_with_crop_or_pad, resize_input
     from .e2eflow.core import tf_image
     rh, rw = dims
@@ -149,14 +158,32 @@ def evaluate_examples(name, items, dims, flow_fn, device, num=10, out_dir=None, 
         for k, v in scalars.items():
             sums[k] = sums.get(k, 0.0) + float(v)
         iterstr = str(n).zfill(6)
-        if output_visual and out_dir:
+        keep_tiles = pages is not None and pages.wants_more()
+        if (output_visual and out_dir) or keep_tiles:
             im1_o = tf_image.resize_bilinear(im1, [h, w])
             im2_o = tf_image.resize_bilinear(im2, [h, w])
-            write_rgb_png(((im1_o * 0.5 + im2_o * 0.5)).cpu().numpy(), os.path.join(out_dir, iterstr + '_img.png'))
-            write_rgb_png((flow_util.flow_to_color(flow) * 255).cpu().numpy(), os.path.join(out_dir, iterstr + '_flow.png'))
+            overlay = im1_o * 0.5 + im2_o * 0.5
+            flow_rgb = flow_util.flow_to_color(flow) * 255
+            err_rgb = None
             if len(truth) == 4:
-                err = flow_util.flow_error_image(flow, truth[0], truth[1], truth[3])
-                write_rgb_png((err * 255).cpu().numpy(), os.path.join(out_dir, iterstr + '_err.png'))
+                err_rgb = flow_util.flow_error_image(flow, truth[0], truth[1], truth[3]) * 255
+            if output_visual and out_dir:
+                write_rgb_png(overlay.cpu().numpy(), os.path.join(out_dir, iterstr + '_img.png'))
+                write_rgb_png(flow_rgb.cpu().numpy(), os.path.join(out_dir, iterstr + '_flow.png'))
+                if err_rgb is not None:
+                    write_rgb_png(err_rgb.cpu().numpy(), os.path.join(out_dir, iterstr + '_err.png'))
+            if keep_tiles:
+                # the image slots of _evaluate_experiment (eval_gui.py:147-204), every value times 255
+                warp_err = torch.abs(im1_o - image_warp(im2_o, flow))
+                if len(truth) == 4:
+                    slots = (('overlay', overlay), ('brightness error', warp_err), ('flow', flow_rgb),
+                             ('flow error', err_rgb))
+                elif len(truth) == 2:
+                    slots = (('overlay', overlay), ('brightness error', warp_err), ('flow', flow_rgb),
+                             ('gt', flow_util.flow_to_color(truth[0], truth[1]) * 255))
+                else:
+                    slots = (('first image', im1_o), ('warp error', warp_err), ('flow prediction', flow_rgb))
+                pages.add([s[0] for s in slots], [to_uint8(s[1]) for s in slots])
         if output_benchmark and out_dir:
             targets = [(flow, '_10')] + ([(flow_bw, '_01')] if output_backward else [])
             for f, suffix in targets:
@@ -199,7 +226,7 @@ def experiment_setup(name, default_config_path, dataset, conv_default=None):
     return params, ckpt, config_path
 
 
-def main(argv=None):
+def arg_parser():
     ap = argparse.ArgumentParser()
     ap.add_argument('--dataset', default='kitti', choices=tuple(DATASETS))
     ap.add_argument('--variant', default='train_2012',
@@ -212,11 +239,22 @@ def main(argv=None):
     ap.add_argument('--output_benchmark', action='store_true', help='Output raw flow files.')
     ap.add_argument('--output_visual', action='store_true', help='Output flow visualization files.')
     ap.add_argument('--output_backward', action='store_true', help='Output backward flow files.')
+    ap.add_argument('--output_pages', action='store_true',
+                    help='Write <out>/pages/%%06d.png: a page per example, a row per image slot and a column '
+                         'per experiment of --ex, as the reference viewer shows them. The tiles are kept in '
+                         'host memory until the last experiment is done: about num_vis x slots (3 or 4) x '
+                         'experiments x height x width x 3 bytes, 1.7 GB for 100 KITTI pages of 3 experiments.')
+    ap.add_argument('--num_vis', type=int, default=100,
+                    help='Number of examples to write pages for. -1 = all. No effect without --output_pages.')
     ap.add_argument('--output_png', dest='output_png', action='store_true', default=True)
     ap.add_argument('--no-output_png', dest='output_png', action='store_false', help='write .flo instead')
     ap.add_argument('--config', default=os.environ.get('UNFLOW_CONFIG', '../config.ini'))
     ap.add_argument('--out', default='../out')
-    args = ap.parse_args(argv)
+    return ap
+
+
+def main(argv=None):
+    args = arg_parser().parse_args(argv)
     check_variant(args.dataset, args.variant)
     if not torch.cuda.is_available():
         raise SystemExit("unflow_b200.eval needs a CUDA device (no CPU fallback)")
@@ -239,8 +277,13 @@ def run_eval(args, device, make_flow_fn=network_flow_fn):
     num = args.num
     if num == -1:
         num = ALL_PAIRS.get((args.dataset, args.variant), num)
-    results = {}
-    for name in [n for n in args.ex.split(',') if n]:
+    names = [n for n in args.ex.split(',') if n]
+    # a namespace built by a caller may predate these two flags
+    output_pages, num_vis = getattr(args, 'output_pages', False), getattr(args, 'num_vis', 100)
+    if output_pages and 'pages' in names and (args.output_visual or args.output_benchmark):
+        raise SystemExit("--output_pages writes <out>/pages, the output directory of experiment 'pages'")
+    results, columns = {}, []
+    for name in names:
         params, ckpt, config_path = experiment_setup(name, args.config, args.dataset, conv_default)
         print("-- evaluating '{}' in conv precision {}".format(name, conv_ops.get_mode()))
         variables = FlowNetVariables(params.get('flownet', 'S'), params.get('full_res'), seed=0).to(device)
@@ -250,6 +293,9 @@ def run_eval(args, device, make_flow_fn=network_flow_fn):
         holder = _Holder()
         holder.variables = variables
         restore_checkpoint(holder, ckpt[1])
+        if output_pages:
+            from .e2eflow.core.pages import Tiles
+            columns.append(Tiles(num_vis))
         out_dir = None
         if args.output_visual or args.output_benchmark:
             out_dir = os.path.join(args.out, name)
@@ -260,7 +306,13 @@ def run_eval(args, device, make_flow_fn=network_flow_fn):
         results[name] = evaluate_examples(
             name, input_fn(), data_input.dims, make_flow_fn(params, data_input.get_normalization(), variables),
             device, num=num, out_dir=out_dir, output_benchmark=args.output_benchmark,
-            output_visual=args.output_visual, output_backward=args.output_backward, output_png=args.output_png)
+            output_visual=args.output_visual, output_backward=args.output_backward, output_png=args.output_png,
+            pages=columns[-1] if output_pages else None)
+    if output_pages:
+        from .e2eflow.core.pages import write_pages
+        title = 'Flow eval: {}/{}'.format(args.dataset, args.variant)
+        write_pages(os.path.join(args.out, 'pages'), lambda i: '{} {:06d}'.format(title, i), names, columns,
+                    threads=os.cpu_count() or 1)
     return results
 
 

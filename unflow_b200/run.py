@@ -74,6 +74,11 @@
   mode only.  ``<[dirs] log>/ex/<name>/eval`` gets the AEE / outlier averages and every tracked loss
   averaged over the evaluation set after every ``save_interval`` chunk, at that iteration.  ``--ow``
   removes both.  View them with ``tensorboard --logdir <[dirs] log>/ex``.
+* [run] interactive_plot = True (train.py:287-308, 378-384): after every in-training evaluation rank 0 writes
+  its pages to ``<[dirs] log>/ex/<name>/eval_pages/%06d.png``, one per evaluated pair, titled
+  ``<name> (i=<iteration>)``, with the rows warped image, flow, occ, reverse disocc and flow error
+  (``core/pages.py``); they replace the previous evaluation's pages, as the reference replaces its plot
+  window.  Also with ``--debug``.  The PNGs are encoded on a background thread while training continues.
 """
 import argparse
 import configparser
@@ -422,12 +427,14 @@ def stage_datasets(data_dir, fast_dir, train_dataset, local_rank=0):
     return stage(data_dir, fast_dir, dirs)
 
 
-def evaluate_kitti(trainer, eval_input, device, hold_out_inv=None, dataset='2012', loss_averages=None):
+def evaluate_kitti(trainer, eval_input, device, hold_out_inv=None, dataset='2012', loss_averages=None,
+                   pages=None):
     """train.py:265-385 on ``einput.input_train_2012()`` (``dataset='2012'``) or
     ``einput.input_train_2015()`` (``'2015'``): every pair is brought back to its file size (the
     queue pads to 384x1280), resized bilinearly to 384x1280 for the network, and the flow is resized
     back before AEE / outlier-% against the occluded and non-occluded ground truth.  ``loss_averages``:
-    a dict that receives the tracked losses averaged over the pairs (core/train.py: evaluate)."""
+    a dict that receives the tracked losses averaged over the pairs, ``pages`` a ``pages.Tiles`` that
+    receives their visualisation tiles (core/train.py: evaluate)."""
     from .e2eflow.core.input import resize_image_with_crop_or_pad
     from .e2eflow.core.train import evaluate
     source = {'2012': eval_input.input_train_2012, '2015': eval_input.input_train_2015}[dataset]
@@ -439,8 +446,14 @@ def evaluate_kitti(trainer, eval_input, device, hold_out_inv=None, dataset='2012
                         for t in (item[0], item[1]) + item[3:])
 
     result, _ = evaluate(trainer.variables, trainer.params, trainer.normalization, examples(),
-                         loss_averages=loss_averages)
+                         loss_averages=loss_averages, pages=pages)
     return result
+
+
+def interactive_plot(run_config):
+    """[run] interactive_plot (train.py:378-384): write the pages of every in-training evaluation.  Off
+    when the key is absent or False."""
+    return bool(run_config.get('interactive_plot', False))
 
 
 def summary_writers(log_dir, name, rank, overwrite=False):
@@ -602,6 +615,12 @@ def main(argv=None):
         print('-- training from i = {} to {}'.format(start_iter, num_iters))
     print('-- rank {}: conv precision {}'.format(rank, precision))
 
+    # rank 0 writes the pages of each evaluation on a background thread; the next evaluation and the end of
+    # the run wait for it and raise its error
+    plots = None
+    if rank == 0 and interactive_plot(run_config):
+        from .e2eflow.core import pages
+        plots = pages.PageWriter()
     batches, eval_input = None, None
     data_dir = dirs.get('data', '')
     if not args.synthetic and os.path.isdir(data_dir):
@@ -633,17 +652,23 @@ def main(argv=None):
                 if not args.debug and rank == 0:
                     save_checkpoint(tr, ckpt_dir, i, args.ckpt_format)
                 if eval_input is not None and rank == 0:      # Trainer.run: self.eval(1) after every chunk
-                    loss_averages = {}
+                    loss_averages, tiles = {}, None
+                    if plots is not None:
+                        plots.join()
+                        tiles = pages.Tiles()
                     if supervised:      # the 2015 pairs input_train_gt held out
                         result = evaluate_kitti(tr, eval_input, device, FT_HOLD_OUT, dataset='2015',
-                                                loss_averages=loss_averages)
+                                                loss_averages=loss_averages, pages=tiles)
                     else:
                         result = evaluate_kitti(tr, eval_input, device, params.get('eval_hold_out_inv'),
-                                                loss_averages=loss_averages)
+                                                loss_averages=loss_averages, pages=tiles)
                     print("-- eval: i = {}".format(i))
                     for k in sorted(result):
                         print("   {} = {}".format(k, result[k]))
                     write_eval_summaries(eval_writer, i, result, loss_averages)
+                    if plots is not None:       # the previous evaluation's pages are replaced (train.py:379-380)
+                        title = "{} (i={})".format(args.ex, i)
+                        plots.start(os.path.join(ex_dir, 'eval_pages'), lambda _, t=title: t, [args.ex], [tiles])
                 if world > 1:
                     # rank 0 alone writes the checkpoint and evaluates: the others wait here instead of inside the
                     # next step's all-reduce (where the wait would run into the NCCL watchdog and count as step time)
@@ -651,6 +676,8 @@ def main(argv=None):
     finally:
         if batches is not None:
             batches.close()
+        if plots is not None:
+            plots.join()
     if rank == 0 and not args.debug:      # after the last chunk's barrier; the other ranks need not wait
         conclude(ckpt_dir, ex_dir)
     for w in (train_writer, eval_writer):
