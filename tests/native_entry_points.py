@@ -126,3 +126,19 @@ VARIANT_STEP_CALLS = {
         "unflow_backward_warp_fwd", "unflow_backward_warp_bwd",
         "unflow_supervised_loss_fwd", "unflow_supervised_loss_bwd", "unflow_supervised_loss_workspace_bytes"},
 }
+
+# The entry points of each case of tests/test_gpu_batch_step_launches.py (384x1280, 3xTF32, default options), as
+# observed on an H100: the FlowNetC step at per-rank batches 1, 2 and 3 and the CSS step at batch 1 call what their
+# batch-4 steps call (the bias + leaky ReLU pass after a K-sliced launch runs inside unflow_tc_conv, not through the
+# handle); the evaluation forward (eval.network_flow_fn) calls the forward half of the FlowNetC step.
+EVAL_FORWARD_CALLS = PLAIN_STEP_CALLS - _CORR_BIDIR_GRAD - {
+    "unflow_adam_step_l2", "unflow_bias_grad_lrelu", "unflow_conv3x3_narrow_wgrad",
+    "unflow_conv3x3_narrow_wgrad_workspace_bytes", "unflow_level_loss_bwd", "unflow_lrelu_bwd_bias",
+    "unflow_tc_wgrad", "unflow_tc_wgrad_window"}
+BATCH_STEP_CALLS = {
+    "C-b1": PLAIN_STEP_CALLS,
+    "C-b2": PLAIN_STEP_CALLS,
+    "C-b3": PLAIN_STEP_CALLS,
+    "CSS-b1": _FROZEN_C_STACK_CALLS,
+    "eval": EVAL_FORWARD_CALLS,
+}

@@ -59,3 +59,11 @@ def test_standalone_entry_points_name_existing_tests():
         body = open(os.path.join(HERE, fname)).read()
         assert name[len("unflow_"):] in body or name in body or fname == "test_gpu_supervised.py", \
             "%s is not exercised in %s" % (name, fname)
+
+
+def test_batch_step_cases_and_pinned_sets_match_the_table():
+    tree = ast.parse(open(os.path.join(HERE, "test_gpu_batch_step_launches.py")).read())
+    assert {k.value for k in _assigned_dict(tree, "CASES").keys} == set(EP.BATCH_STEP_CALLS)
+    checked = set(EP.STEP_CHECKED) | set(EP.VARIANT_CHECKED) | set(EP.TC_DELEGATED) | set(EP.HOST_ONLY)
+    for cid, pinned in EP.BATCH_STEP_CALLS.items():
+        assert pinned <= checked, "%s calls entry points without a checker: %s" % (cid, sorted(pinned - checked))

@@ -31,39 +31,49 @@ def plan(N, Hin, Win, Cin, Hout, Wout, Cout, mode, stride, kh, kw, pt, pl):
     return p
 
 
+def tile_boxes(p):
+    """(n, iy, ix) [tiles, TN*TH*TW] of every element of every tile box: tile (tn, ty, tx) starts at
+    (tn * TN, ty * TH, tx * TW) of the iteration space; elements past its end are part of the box too."""
+    TW, TH, TN = p["TW"], p["TH"], p["TN"]
+    tn, ty, tx = torch.meshgrid(torch.arange(p["tiles_n"]), torch.arange(p["tiles_y"]), torch.arange(p["tiles_x"]),
+                                indexing="ij")
+    a, b, c = torch.meshgrid(torch.arange(TN), torch.arange(TH), torch.arange(TW), indexing="ij")
+    return (tn.reshape(-1, 1) * TN + a.reshape(1, -1), ty.reshape(-1, 1) * TH + b.reshape(1, -1),
+            tx.reshape(-1, 1) * TW + c.reshape(1, -1))
+
+
+def load_box(x, n, yy, xx):
+    """The TMA box: x[n, yy, xx] per element, zero fill outside the tensor."""
+    N, Hin, Win, Cin = x.shape
+    box = torch.zeros(n.shape + (Cin,), dtype=x.dtype)
+    ok = (n < N) & (yy >= 0) & (yy < Hin) & (xx >= 0) & (xx < Win)
+    box[ok] = x[n[ok], yy[ok], xx[ok]]
+    return box
+
+
+def store_box(out, written, acc, p, n, iy, ix, py, px, s_out):
+    """The epilogue: box elements inside the iteration space go to out[n, s_out*iy + py, s_out*ix + px]."""
+    keep = (n < out.shape[0]) & (iy < p["Hit"]) & (ix < p["Wit"])
+    idx = (n[keep], s_out * iy[keep] + py, s_out * ix[keep] + px)
+    out[idx] = acc[keep]
+    written.index_put_(idx, torch.ones(len(idx[0]), dtype=written.dtype), accumulate=True)
+
+
 def execute(p, x, w_taps, N, Hout, Wout, Cout):
-    """x [N,Hin,Win,Cin] (NHWC), w_taps [taps][Cout][Cin]; tile by tile like the kernel."""
-    _, Hin, Win, Cin = x.shape
+    """x [N,Hin,Win,Cin] (NHWC), w_taps [taps][Cout][Cin]; tile by tile like the kernel (all tiles of a class
+    at once)."""
     out = torch.full((N, Hout, Wout, Cout), float("nan"), dtype=x.dtype)
     written = torch.zeros((N, Hout, Wout), dtype=torch.int32)
-    TW, TH, TN = p["TW"], p["TH"], p["TN"]
-    assert TW * TH * TN <= 128
+    assert p["TW"] * p["TH"] * p["TN"] <= 128
+    n, iy, ix = tile_boxes(p)
     for cls in range(p["n_classes"]):
         px, py = p["class_pxy"][cls]
         taps = p["taps"][p["class_start"][cls]:p["class_start"][cls + 1]]
-        for tn in range(p["tiles_n"]):
-            for ty in range(p["tiles_y"]):
-                for tx in range(p["tiles_x"]):
-                    n0, iy0, ix0 = tn * TN, ty * TH, tx * TW
-                    acc = torch.zeros((TN, TH, TW, Cout), dtype=x.dtype)
-                    for (dx, dy, widx) in taps:
-                        # the TMA box: element stride s_in, zero fill outside the tensor
-                        box = torch.zeros((TN, TH, TW, Cin), dtype=x.dtype)
-                        for a in range(TN):
-                            for b in range(TH):
-                                for c in range(TW):
-                                    n, yy, xx = n0 + a, p["s_in"] * (iy0 + b) + dy, p["s_in"] * (ix0 + c) + dx
-                                    if n < N and 0 <= yy < Hin and 0 <= xx < Win:
-                                        box[a, b, c] = x[n, yy, xx]
-                        acc += box @ w_taps[widx].t()
-                    for a in range(TN):
-                        for b in range(TH):
-                            for c in range(TW):
-                                n, iy, ix = n0 + a, iy0 + b, ix0 + c
-                                if n < N and iy < p["Hit"] and ix < p["Wit"]:
-                                    oy, ox = p["s_out"] * iy + py, p["s_out"] * ix + px
-                                    out[n, oy, ox] = acc[a, b, c]
-                                    written[n, oy, ox] += 1
+        acc = torch.zeros(n.shape + (Cout,), dtype=x.dtype)
+        for (dx, dy, widx) in taps:
+            # element stride s_in
+            acc += load_box(x, n, p["s_in"] * iy + dy, p["s_in"] * ix + dx) @ w_taps[widx].t()
+        store_box(out, written, acc, p, n, iy, ix, py, px, p["s_out"])
     assert int(written.min()) == 1 and int(written.max()) == 1     # every output exactly once
     return out
 
@@ -261,43 +271,24 @@ def execute_pair_px(p, x, w_taps, N, Hout, Wout, Cout):
     """The two-parity-classes-per-tile form (csrc/tc_conv.cu, pair_px_plan): a class = an output ROW parity, a
     tile computes 2 * Cout virtual columns -- [0, Cout) the channels of px = 0 with tap widx, [Cout, 2 Cout) those
     of px = 1 with tap widx2; -1 = that class has no tap for the input offset (zero weights)."""
-    _, Hin, Win, Cin = x.shape
     out = torch.full((N, Hout, Wout, Cout), float("nan"), dtype=x.dtype)
     written = torch.zeros((N, Hout, Wout), dtype=torch.int32)
-    TW, TH, TN = p["TW"], p["TH"], p["TN"]
     assert p["pair_px"] == 1 and p["n_classes"] == 2 and p["n_blocks"] == 1 and p["BN"] == 128 and p["s_out"] == 2
+    n, iy, ix = tile_boxes(p)
     for cls in range(2):
         py = p["class_pxy"][cls][1]
-        lo, hi = p["class_start"][cls], p["class_start"][cls + 1]
-        for tn in range(p["tiles_n"]):
-            for ty in range(p["tiles_y"]):
-                for tx in range(p["tiles_x"]):
-                    n0, iy0, ix0 = tn * TN, ty * TH, tx * TW
-                    acc = torch.zeros((TN, TH, TW, 2 * Cout), dtype=x.dtype)
-                    for ti in range(lo, hi):
-                        dx, dy, widx = p["taps"][ti]
-                        widx2 = p["widx2"][ti]
-                        assert widx >= 0 or widx2 >= 0
-                        box = torch.zeros((TN, TH, TW, Cin), dtype=x.dtype)
-                        for a in range(TN):
-                            for b in range(TH):
-                                for c in range(TW):
-                                    n, yy, xx = n0 + a, iy0 + b + dy, ix0 + c + dx
-                                    if n < N and 0 <= yy < Hin and 0 <= xx < Win:
-                                        box[a, b, c] = x[n, yy, xx]
-                        if widx >= 0:
-                            acc[..., :Cout] += box @ w_taps[widx].t()
-                        if widx2 >= 0:
-                            acc[..., Cout:] += box @ w_taps[widx2].t()
-                    for a in range(TN):
-                        for b in range(TH):
-                            for c in range(TW):
-                                n, iy, ix = n0 + a, iy0 + b, ix0 + c
-                                if n < N and iy < p["Hit"] and ix < p["Wit"]:
-                                    for px in range(2):
-                                        oy, ox = 2 * iy + py, 2 * ix + px
-                                        out[n, oy, ox] = acc[a, b, c, px * Cout:(px + 1) * Cout]
-                                        written[n, oy, ox] += 1
+        acc = torch.zeros(n.shape + (2 * Cout,), dtype=x.dtype)
+        for ti in range(p["class_start"][cls], p["class_start"][cls + 1]):
+            dx, dy, widx = p["taps"][ti]
+            widx2 = p["widx2"][ti]
+            assert widx >= 0 or widx2 >= 0
+            box = load_box(x, n, iy + dy, ix + dx)
+            if widx >= 0:
+                acc[..., :Cout] += box @ w_taps[widx].t()
+            if widx2 >= 0:
+                acc[..., Cout:] += box @ w_taps[widx2].t()
+        for px in range(2):
+            store_box(out, written, acc[..., px * Cout:(px + 1) * Cout], p, n, iy, ix, py, px, 2)
     assert int(written.min()) == 1 and int(written.max()) == 1
     return out
 
