@@ -1,10 +1,11 @@
 """Float64 references of the non-tensor-core kernels (include/unflow.h), with their error scales.
 
-Every reference here is the operation's definition evaluated in float64 on the GPU from the float32 operands the
-kernel read.  Each comes with A, the same evaluation on absolute values (every difference becomes a sum of
-magnitudes), so that a kernel is checked elementwise as |got - ref| <= TAU * A: an error cannot hide behind
+Every reference here is the operation's definition evaluated in float64 from the float32 operands the kernel read,
+on the device of its operands.  Each comes with A, the same evaluation on absolute values (every difference becomes
+a sum of magnitudes), so that a kernel is checked elementwise as |got - ref| <= TAU * A: an error cannot hide behind
 cancellation or behind a large element elsewhere.  Used by tests/test_gpu_step_launches.py (one training step,
-every launch) and tests/test_gpu_float64_kernels.py (the shapes and edges the step does not reach).
+every launch) and tests/test_gpu_float64_kernels.py (the shapes and edges the step does not reach); pinned on the
+CPU to the reference's golden outputs, the oracle and brute definitions by tests/test_float64_refs_cpu.py.
 """
 import math
 
@@ -258,6 +259,7 @@ def forward_warp_grads(grad, flow):
 
 # ---- the fused level loss (csrc/level_loss.cu; reference losses.py:16-122,206-366) ---------------------------------
 EPS2, ALPHA = 1e-6, 0.45
+FB_OCC_OFFSET = 0.5         # the fb occlusion test |f + w(g)|^2 > 0.01 (|f|^2 + |w(g)|^2) + 0.5 (losses.py:59-63)
 TERMS = ['sym', 'occ', 'photo', 'grad', 'smooth_1st', 'smooth_2nd', 'fb', 'ternary']
 
 
@@ -327,7 +329,7 @@ def _first_order_deltas(f):
 
 
 class LevelInputs:
-    """The operands of one level-loss call as float64 GPU tensors (flows [B,h,w,2], masks [B,h,w])."""
+    """The operands of one level-loss call as float64 tensors (flows [B,h,w,2], masks [B,h,w])."""
 
     def __init__(self, im1, im2, ffw, fbw, border, fwarp_fw, fwarp_bw, occl, R, bits):
         d = lambda t: None if t is None else t.detach().double()
@@ -343,7 +345,9 @@ class LevelInputs:
 
 def masks_f32(ffw, fbw, border, occl, fwarp_fw, fwarp_bw):
     """mask_fw, mask_bw [B,h,w] by the mask formulas of oracle/losses.py compute_losses, op by op in float32
-    (one rounding per op, no contraction: what the kernel evaluates with __fmul_rn / __fadd_rn)."""
+    (one rounding per op, no contraction: what the kernel evaluates with __fmul_rn / __fadd_rn), on the flows'
+    device."""
+    ffw_in = ffw
     ffw, fbw = ffw.detach().float().cpu(), fbw.detach().float().cpu()
     if border is None:
         mfw, mbw = olosses.create_outgoing_mask(ffw), olosses.create_outgoing_mask(fbw)
@@ -354,19 +358,23 @@ def masks_f32(ffw, fbw, border, occl, fwarp_fw, fwarp_bw):
         occ = []
         for f, gw in ((ffw, fbw_w), (fbw, ffw_w)):
             mag = olosses.length_sq(f) + olosses.length_sq(gw)
-            occ.append((olosses.length_sq(f + gw) > 0.01 * mag + 0.5).float())
+            occ.append((olosses.length_sq(f + gw) > 0.01 * mag + FB_OCC_OFFSET).float())
         mfw, mbw = mfw * (1 - occ[0]), mbw * (1 - occ[1])
     elif occl == 2:
         mfw = mfw * (1 - (fwarp_bw.float().cpu() < 0.8).float())
         mbw = mbw * (1 - (fwarp_fw.float().cpu() < 0.8).float())
-    return mfw[..., 0].cuda(), mbw[..., 0].cuda()
+    dev = ffw_in.device
+    return mfw[..., 0].to(dev), mbw[..., 0].to(dev)
 
 
 def level_losses(L, ffw, fbw, mfw, mbw, variant=None):
     """The 8 loss terms (TERMS order; unrequested ones 0) in float64 with the masks held fixed, differentiable
     w.r.t. ffw and fbw.  variant: None = the definition; 'detach_fb' stops the gradient of the fb term into
     the other flow (through image_warp(flow_bw, flow_fw)); 'clamp_census' replicates the image border in the
-    census window; 'margin' shrinks the census transform mask to R - 1 (wrong kernels, negative controls)."""
+    census window; 'margin' shrinks the census transform mask to R - 1 (wrong kernels, negative controls).
+    The Sobel 'grad' term has no kernel and no reference here: its bit raises."""
+    if L.want('grad'):
+        raise ValueError("level_losses: the 'grad' term is not evaluated")
     B, h, w, R = L.B, L.h, L.w, L.R
     n1 = float(B * h * w)
     out = [ffw.new_zeros(())] * 8
@@ -495,12 +503,13 @@ def level_loss_grad_scale(L, mfw, mbw, gl):
 # ---- the fused supervised flow loss (csrc/supervised_loss.cu; reference supervised.py:45-57) ---------------------
 @torch.enable_grad()        # also inside a backward pass, where autograd is off
 def supervised_loss_grads(flow, gt, mask, scale=20.0):
-    """float64 loss, d loss / d flow, and the elementwise error budget of the float32 kernel's dflow."""
-    from unflow_b200.e2eflow.core import tf_image
+    """float64 loss, d loss / d flow, and the elementwise error budget of the float32 kernel's dflow.  The upscale
+    is the oracle's restatement of TF's legacy resize_bilinear, not the product's."""
+    from oracle import tf_compat
     f32 = 2.0 ** -24
     H, W = gt.shape[1:3]
     f = flow.detach().double().requires_grad_(True)
-    v = tf_image.resize_bilinear(f, (H, W)) * scale
+    v = tf_compat.resize_bilinear_legacy(f, (H, W)) * scale
     x = v - gt.double()
     m = torch.ones_like(x[..., :1]) if mask is None else mask.double()
     n = float(x.numel())

@@ -324,7 +324,7 @@ def test_adam_entry_points_vs_float64(entry, step):
     mask = torch.randint(0, 16, (n // 4,), device="cuda", generator=g, dtype=torch.uint8)
     # the hyper-parameters are fp32 in the ABI: the reference takes the same fp32 values (1 - 0.999f is not 0.001)
     lr, b1, b2, eps, gs, l2 = (float(np.float32(x)) for x in (1e-4, 0.9, 0.999, 1e-8, 0.5, 4e-4))
-    l2m = l2_bits(mask.data_ptr(), n) if entry.endswith("l2") else torch.zeros(n, device="cuda", dtype=torch.float64)
+    l2m = l2_bits(mask, n) if entry.endswith("l2") else torch.zeros(n, device="cuda", dtype=torch.float64)
     (p1, m1, v1), (Ap, Am, Av) = adam_reference(p.double(), gr.double(), m.double(), v.double(), lr, b1, b2, eps, gs,
                                                  float(step), l2m, l2 if entry.endswith("l2") else 0.0)
     ptrs = (p.data_ptr(), gr.data_ptr(), m.data_ptr(), v.data_ptr(), n)

@@ -236,8 +236,16 @@ def test_interactive_plot_data_parallel_rank_0_writes(kitti_tree):
 
 
 # ---- what the pages add to the evaluation loops ------------------------------------------------------
-def profile_counts(fn):
-    """(device-to-host copies, kernels) ``fn`` runs, from torch.profiler."""
+def profile_counts(make, reps=3):
+    """(device-to-host copies, kernels) of the GPU work ``make()`` runs, from torch.profiler: per count, the
+    median of ``reps`` sessions, each running a fresh ``make()`` (a page collector fills up).  A session can
+    miss activities issued right at its start, or take in records of the work before it; the median is the
+    count of a session that did neither."""
+    runs = [_profile_once(make()) for _ in range(reps)]
+    return tuple(sorted(c)[reps // 2] for c in zip(*runs))
+
+
+def _profile_once(fn):
     from torch.autograd import DeviceType
     from torch.profiler import ProfilerActivity, profile
     torch.cuda.synchronize()
@@ -264,7 +272,7 @@ def test_pages_add_one_copy_per_paged_example_and_nothing_when_off(trees):
         return lambda: E.evaluate_examples("w", items, data_input.dims, fn, torch.device("cuda"), num=2,
                                            pages=collector, log=open(os.devnull, "w"))
     eval_loop(pages.Tiles(2))()        # warm-up of every shape
-    off, idle, on = (profile_counts(eval_loop(t)) for t in (None, pages.Tiles(0), pages.Tiles(1)))
+    off, idle, on = (profile_counts(lambda k=k: eval_loop(None if k is None else pages.Tiles(k))) for k in (None, 0, 1))
     print("eval loop, 2 pairs: (copies, kernels) off %s, collector full %s, one page %s" % (off, idle, on))
     assert idle == off
     assert on[0] == off[0] + 1 and on[1] > off[1]
@@ -278,7 +286,7 @@ def test_pages_add_one_copy_per_paged_example_and_nothing_when_off(trees):
     def train_eval(collector):
         return lambda: evaluate(v, dict(synth.KITTI_PARAMS), synth.KITTI_NORMALIZATION, examples, pages=collector)
     train_eval(pages.Tiles())()
-    off, on = profile_counts(train_eval(None)), profile_counts(train_eval(pages.Tiles()))
+    off, on = profile_counts(lambda: train_eval(None)), profile_counts(lambda: train_eval(pages.Tiles()))
     print("training evaluation, 2 pairs: (copies, kernels) off %s, pages %s" % (off, on))
     assert on[0] == off[0] + 2 and on[1] > off[1]
     collected = pages.Tiles()

@@ -52,9 +52,10 @@ def _round4(c):
 
 
 def tf32_rna(w):
-    """fp32 -> the nearest TF32 value (10 mantissa bits, ties away from zero: cvt.rna.tf32.f32), as fp32."""
+    """fp32 -> the nearest TF32 value (10 mantissa bits, ties away from zero: cvt.rna.tf32.f32), as fp32.  A NaN
+    stays a NaN (the carry out of a large payload would wrap it to a signed zero)."""
     b = w.view(torch.int32)
-    return ((b + 0x1000) & ~0x1FFF).view(torch.float32)
+    return torch.where(torch.isnan(w), w, ((b + 0x1000) & ~0x1FFF).view(torch.float32))
 
 
 # ---- checkers: check(args, call) runs the real call via call() and returns a list of (label, shape, ratio, tau) ----
@@ -236,8 +237,9 @@ def adam_reference(p, g, m, v, lr, b1, b2, eps, gs, t, l2m, l2):
     return (p - step, m1, v1), (Ap, Am, Av)
 
 
-def l2_bits(mask_p, n):
-    mk = R.view(mask_p, (n // 4,), dtype=torch.uint8).long()
+def l2_bits(mask, n):
+    """The adam kernel's L2 mask (uint8 [n / 4], bit k of byte i = element 4 * i + k) as float64 flags [n]."""
+    mk = mask.long()
     return torch.stack([(mk >> k) & 1 for k in range(4)], 1).reshape(n).double()
 
 
@@ -247,7 +249,7 @@ def check_adam_l2(a, call):
     p, g, m, v = (b.double() for b in bufs)
     call()
     f32 = lambda x: float(torch.tensor(x, dtype=torch.float32))        # the ABI passes fp32 hyper-parameters
-    l2m = l2_bits(mask_p, n) if mask_p else torch.zeros_like(p)
+    l2m = l2_bits(R.view(mask_p, (n // 4,), dtype=torch.uint8), n) if mask_p else torch.zeros_like(p)
     (p1, m1, v1), (Ap, Am, Av) = adam_reference(p, g, m, v, f32(lr), f32(b1), f32(b2), f32(eps), f32(gs),
                                                  float(step), l2m, f32(l2))
     shape = "n=%d step %d" % (n, step)

@@ -202,11 +202,13 @@ def test_run_kitti_ft_writes_summaries_and_images(tmp_path, capsys):
     assert "loss/combined_2" in ev_acc.Tags()["scalars"]
 
 
-def _step_profile(fn, reps=2):
-    """(kernels, device-to-host copies, other copies) of the GPU work ``fn`` issues: the largest count
-    of ``reps`` profiling sessions of one call each (a session can miss an activity issued right at
-    its start)."""
-    return tuple(max(c) for c in zip(*(_profile_once(fn) for _ in range(reps))))
+def _step_profile(fn, reps=3):
+    """(kernels, device-to-host copies, other copies) of the GPU work ``fn`` issues: per count, the median
+    of ``reps`` profiling sessions of one call each.  A session can miss activities issued right at its
+    start, or take in records of the work before it; the median is the count of a session that did
+    neither."""
+    runs = [_profile_once(fn) for _ in range(reps)]
+    return tuple(sorted(c)[reps // 2] for c in zip(*runs))
 
 
 def _profile_once(fn):
