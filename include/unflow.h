@@ -231,7 +231,8 @@ int unflow_adam_step(float *params, float *grads, float *m, float *v, long long 
                      int zero_grad, void *stream);
 /* Same update with the hyper-parameters read from DEVICE memory at run time:
  * hyper = [lr, beta1, beta2, eps, grad_scale, step]; lr_t is computed on the device from `step`
- * (1 for the first update), which a one-thread kernel advances after the update.  Lets a CUDA graph
+ * (1 for the first update), in double as unflow_adam_step forms it on the host.  A one-thread kernel
+ * advances `step` after the update.  Lets a CUDA graph
  * of the whole training step be replayed without per-step host writes. */
 int unflow_adam_step_dev(float *params, float *grads, float *m, float *v, long long n,
                          float *hyper, int zero_grad, void *stream);

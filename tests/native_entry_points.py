@@ -106,6 +106,17 @@ PLAIN_STEP_CALLS = frozenset((
 ))
 AUGMENT_STEP_CALLS = PLAIN_STEP_CALLS | {"unflow_backward_warp_fwd"}     # the BORDER_STN sampler
 
+
+def captured(calls):
+    """The entry points of a step captured by Trainer.capture whose eager step calls ``calls``: Adam reads its
+    hyper-parameters and step counter from device memory (unflow_adam_step_dev_l2), everything else is the same."""
+    return frozenset(calls - {"unflow_adam_step_l2"} | {"unflow_adam_step_dev_l2"})
+
+
+# The entry points Trainer.capture's warm-ups and captured step call for the FlowNetC step above, as observed on
+# an H100; tests/test_gpu_float64_captured_step.py asserts them (and captured() of the other sets for its other cases).
+CAPTURED_STEP_CALLS = captured(PLAIN_STEP_CALLS)
+
 # The entry points one eager step of each configuration of tests/test_gpu_variant_step_launches.py calls (3xTF32,
 # default options), as observed on an H100; that test asserts them as test_gpu_step_launches.py asserts the sets above.
 _CORR_BIDIR = frozenset(("unflow_correlation_fwd_bidir", "unflow_correlation_fwd_path", "unflow_correlation_out_shape",

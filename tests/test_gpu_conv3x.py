@@ -24,7 +24,9 @@ def _no_library_conv(name, real):
 
 @pytest.fixture
 def mode3x(monkeypatch):
-    from unflow_b200.e2eflow.core import conv_ops
+    # importing flownet sets the mode from UNFLOW_CONV_PRECISION: before set_mode, so that a test which is the first
+    # to import it still runs in 3xtf32
+    from unflow_b200.e2eflow.core import conv_ops, flownet  # noqa: F401
     for mod, name in ((F, "conv2d"), (F, "conv_transpose2d"), (torch.nn.grad, "conv2d_weight")):
         monkeypatch.setattr(mod, name, _no_library_conv(name, getattr(mod, name)))
     old = conv_ops.get_mode()

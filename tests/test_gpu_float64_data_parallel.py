@@ -196,12 +196,13 @@ def _unpack(packed):
     return torch.from_numpy(np.unpackbits(bits.numpy(), count=n).astype(bool)).view(shape).cuda()
 
 
-def _record_decisions(m, Trainer, supervised):
-    """The recorders of the objective file (leaky-ReLU sides; the level-loss calls' flows, masks and splat maps)
-    on the product, emptied at the start of every loss evaluation: after a step they hold that step's decisions.
-    In a captured step they are graph memory, which every replay rewrites."""
+def _record_decisions(m, Trainer, supervised, augment=False):
+    """The recorders of the objective file (leaky-ReLU sides; the level-loss calls' flows, masks and splat maps;
+    under ``augment`` the augmented images and mask) on the product, emptied at the start of every loss evaluation:
+    after a step they hold that step's decisions.  In a captured step they are graph memory, which every replay
+    rewrites."""
     sides = R.record_kink_sides(m)
-    rec = None if supervised else _record_loss_side(m, False)
+    rec = None if supervised else _record_loss_side(m, augment)
     real = Trainer.loss
 
     def loss(self, *batch):
@@ -300,26 +301,38 @@ def _product_layout(name, t):
 
 
 def _cases(cid):
-    params, B, H, W, supervised = CASES[cid]
+    return _case_tuples(*CASES[cid])
+
+
+def _case_tuples(params, B, H, W, supervised, augment=False):
     ncase = (params['flownet'], params.get('train_all'), False, False, B, H, W, "supervised", "flat", 1)
-    return params, supervised, ncase, (params, B, H, W, False)
+    return params, supervised, ncase, (params, B, H, W, augment)
 
 
 def shard_reference(monkeypatch, cid, tfv, batch, sides, rec):
     """{name: float64 gradient} (L2 term included, the product's layout) of the case's objective on one shard at the
     variables ``tfv``, following the decisions ``sides`` / ``rec`` the data-parallel step recorded on that shard."""
-    params, supervised, ncase, ocase = _cases(cid)
+    return float64_objective(monkeypatch, CASES[cid], tfv, batch, sides, rec)[1]
+
+
+def float64_objective(monkeypatch, case, tfv, batch, sides, rec, augment=False):
+    """(float64 loss or None for the supervised loss, {name: float64 gradient}) of ``case`` = (loss parameters, B,
+    H, W, supervised) on ``batch`` at the variables ``tfv``, following the recorded decisions ``sides`` / ``rec``
+    (with ``augment``, the recorded augmented images and mask)."""
+    params, supervised, ncase, ocase = _case_tuples(*case, augment=augment)
     rec = _to(rec, "cuda")
+    loss = None
     with monkeypatch.context() as m:
         used, cat = R.follow_kink_sides(m, sides)
         if supervised:
             _, ref = N.run_oracle(m, ncase, tfv, [batch])
         else:
-            _, ref, log = run_float64(m, ocase, tfv, batch, rec)
+            out, ref, log = run_float64(m, ocase, tfv, batch, rec)
             assert len(log) == len(rec.levels), "level-loss calls the oracle did not make"
             assert_case(params, {}, log, [])     # the recorded mask bits are the right ones
+            loss = out["loss"]
     assert all(used[k] == cat[k].shape[0] for k in cat), "activations the oracle did not consume"
-    return ref
+    return loss, ref
 
 
 def single_gpu_run(monkeypatch, cid, tfv, batch):
@@ -342,39 +355,49 @@ def _score(got, ref):
     return rows
 
 
-def effective_gradients(states):
-    """{step: {name: g_eff}} in the product's layout, float64, from the first moments of steps 1 and 2."""
+def _moments_before(states, i, name):
+    """(m, v) of ``name`` after step i - 1, float64: zeros before the first step (no slot recorded)."""
+    prev = states[i - 1].get("slots") or {}
+    if name not in prev:
+        return 0.0, 0.0
+    return tuple(t.double() for t in prev[name])
+
+
+def effective_gradients(states, steps=(1, 2)):
+    """{step: {name: g_eff}} in the product's layout, float64, from the first moments of ``steps`` and of the
+    step before each: g_i = (m_i - b1 m_(i-1)) / (1 - b1)."""
     b1 = float(torch.tensor(0.9, dtype=torch.float32))
     c1 = float(torch.tensor(1.0) - torch.tensor(0.9))       # 1 - b1 as the kernel forms it: 0.100000024
-    out = {1: {}, 2: {}}
-    for name, (m1, _) in states[1]["slots"].items():
-        m1, m2 = m1.double(), states[2]["slots"][name][0].double()
-        out[1][name] = _product_layout(name, m1 / c1).cuda()
-        out[2][name] = _product_layout(name, (m2 - b1 * m1) / c1).cuda()
+    out = {i: {} for i in steps}
+    for i in steps:
+        for name, (m, _) in states[i]["slots"].items():
+            m_prev = _moments_before(states, i, name)[0]
+            out[i][name] = _product_layout(name, (m.double() - b1 * m_prev) / c1).cuda()
     return out
 
 
-def moment_errors(states):
-    """Worst |v_i - v_i(g_i)| over steps and elements, in units of 2^-24 |v| (2^-126 at least)."""
+def moment_errors(states, steps=(1, 2)):
+    """Worst |v_i - v_i(g_i)| over ``steps`` and elements, in units of 2^-24 |v| (2^-126 at least)."""
     b1, b2 = (float(torch.tensor(b, dtype=torch.float32)) for b in (0.9, 0.999))
     c1, c2 = (float(torch.tensor(1.0) - torch.tensor(b)) for b in (0.9, 0.999))
     worst = 0.0
-    for name, (m1, v1) in states[1]["slots"].items():
-        m2, v2 = states[2]["slots"][name]
-        m1, v1, m2, v2 = (t.double() for t in (m1, v1, m2, v2))
-        g1, g2 = m1 / c1, (m2 - b1 * m1) / c1
-        for got, want in ((v1, c2 * g1 * g1), (v2, b2 * v1 + c2 * g2 * g2)):
-            err = (got - want).abs() / (F32 * want.abs().clamp_min(2.0 ** -126))
+    for i in steps:
+        for name, (m, v) in states[i]["slots"].items():
+            m_prev, v_prev = _moments_before(states, i, name)
+            m, v = m.double(), v.double()
+            g = (m - b1 * m_prev) / c1
+            want = b2 * v_prev + c2 * g * g
+            err = (v - want).abs() / (F32 * want.abs().clamp_min(2.0 ** -126))
             worst = max(worst, float(err.max()))
     return worst
 
 
-def update_errors(states, params):
-    """Worst |p_i - p_i(Adam)| over steps 1, 2 and elements, in units of 2^-24 (|p_i| + |update|)."""
+def update_errors(states, params, steps=(1, 2)):
+    """Worst |p_i - p_i(Adam)| over ``steps`` and elements, in units of 2^-24 (|p_i| + |update|)."""
     from unflow_b200.e2eflow.core.train import learning_rate_at
     b1, b2, eps = (float(torch.tensor(b, dtype=torch.float32)) for b in (0.9, 0.999, 1e-8))
     worst = 0.0
-    for i in (1, 2):
+    for i in steps:
         lr_t = learning_rate_at(i - 1, params) * (1 - b2 ** i) ** 0.5 / (1 - b1 ** i)
         for name, (m, v) in states[i]["slots"].items():
             p0, p1 = states[i - 1]["vars"][name].double(), states[i]["vars"][name].double()

@@ -61,6 +61,20 @@ def test_standalone_entry_points_name_existing_tests():
             "%s is not exercised in %s" % (name, fname)
 
 
+def test_captured_step_calls_match_the_eager_step():
+    """The captured step calls what the eager step calls, with Adam on device hyper-parameters instead of host ones;
+    the device Adam has its own float64 test, and the captured step file pins these sets."""
+    assert EP.CAPTURED_STEP_CALLS - EP.PLAIN_STEP_CALLS == {"unflow_adam_step_dev_l2"}
+    assert EP.PLAIN_STEP_CALLS - EP.CAPTURED_STEP_CALLS == {"unflow_adam_step_l2"}
+    assert "unflow_adam_step_dev_l2" in EP.STANDALONE and "unflow_adam_step_l2" in EP.STEP_CHECKED
+    checked = set(EP.STEP_CHECKED) | set(EP.TC_DELEGATED) | set(EP.HOST_ONLY)
+    assert EP.CAPTURED_STEP_CALLS - {"unflow_adam_step_dev_l2"} <= checked
+    for calls in (EP.AUGMENT_STEP_CALLS, *EP.VARIANT_STEP_CALLS.values()):
+        assert EP.captured(calls) ^ calls <= {"unflow_adam_step_l2", "unflow_adam_step_dev_l2"}
+    tree = ast.parse(open(os.path.join(HERE, "test_gpu_float64_captured_step.py")).read())
+    assert "CAPTURED_STEP_CALLS" in ast.dump(_assigned_dict(tree, "CASES")), "no captured case pins the set"
+
+
 def test_batch_step_cases_and_pinned_sets_match_the_table():
     tree = ast.parse(open(os.path.join(HERE, "test_gpu_batch_step_launches.py")).read())
     assert {k.value for k in _assigned_dict(tree, "CASES").keys} == set(EP.BATCH_STEP_CALLS)

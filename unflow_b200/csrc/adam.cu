@@ -30,8 +30,10 @@ adam_kernel(float4 *__restrict__ p, float4 *__restrict__ g, float4 *__restrict__
   if (hyper) {
     b1 = __ldg(hyper + 1); b2 = __ldg(hyper + 2); eps = __ldg(hyper + 3);
     grad_scale = __ldg(hyper + 4);
-    const float t = __ldg(hyper + 5);
-    lr_t = __ldg(hyper) * sqrtf(1.0f - powf(b2, t)) / (1.0f - powf(b1, t));
+    // in double, as unflow_adam_step_l2 forms it on the host: in fp32, 1 - powf(0.999f, t) cancels the rounding
+    // of the power into a 3e-6 error of lr_t from t = 2 on
+    const double t = __ldg(hyper + 5);
+    lr_t = (float)((double)__ldg(hyper) * sqrt(1.0 - pow((double)b2, t)) / (1.0 - pow((double)b1, t)));
   }
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n4;
        i += (long long)gridDim.x * blockDim.x) {
